@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the MCVD DDPM-sampling hot path on B200.
+"""Benchmark of the MCVD DDPM-sampling hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torch.distributed.run)
     python bench.py --impl reference ...                      (CPU arm: the reference algorithm on host cores)
@@ -9,12 +9,12 @@ final denoise evaluation + L fused updates (models/__init__.py:207-340 in the re
 ``ddpm_sampler`` call; it produces B * num_frames frames.  With ``--ar`` a step is the whole autoregressive
 ``video_gen`` loop of the reference (runners/ncsn_runner.py:1501-1570): ceil(num_frames_pred / num_frames) sampler
 calls with the sliding conditioning window, num_frames_pred kept frames per clip.
-Default workload = BASELINE.json configs[1] ("cfg2": smmnist_DDPM_big5 + ngf=96, batch 64, subsample 100,
+Default workload = "cfg2" (mcvd_b200/configs.py: smmnist_DDPM_big5 + ngf=96, batch 64, subsample 100,
 64x64x1, concat conditioning).
 Multi-GPU: every rank owns its OWN clips (global clip ids, distinct synthetic data, noise keyed by the global
 clip id), no data-path collective, and ONE NCCL all-gather of the finished frames, which is inside the e2e timed
 region together with the host<->device copies.  ``--scaling weak`` (default): ``batch`` clips per GPU;
-``--scaling strong``: the workload's batch split over the GPUs (BASELINE: cfg4 on 4, cfg5 on 8).
+``--scaling strong``: the workload's batch split over the GPUs (workloads in mcvd_b200/configs.py; e.g. cfg4 on 4, cfg5 on 8).
 
 Prints ONE JSON line on rank 0 (see the keys at the bottom).
 """
@@ -68,6 +68,9 @@ def parse():
     ap.add_argument("--ar", action="store_true", help="time the full autoregressive video_gen loop (num_frames_pred frames)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
     ap.add_argument("--cpu-batch", type=int, default=0, help="clips per CPU-arm step (0 = 2, or 1 when --steps > 5)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the frames the last timed step produced to DIR/frames.npy (float32; with several GPUs, "
+                         "rank 0's clips)")
     ap.add_argument("--psnr-steps", type=int, default=0, help="DDPM steps of the PSNR check (default: the workload's)")
     return ap.parse_args()
 
@@ -115,7 +118,7 @@ class ClockSampler:
 
 # ------------------------------------------------------------------------------------------------ flops
 def algorithmic_gflop_per_forward(cfg) -> float:
-    """conv + matmul FLOPs (2 per MAC) of ONE sample-forward on the reference graph (BASELINE.md table)."""
+    """conv + matmul FLOPs (2 per MAC) of ONE sample-forward on the reference graph."""
     from mcvd_b200 import arch
     ns = arch.build_spec(cfg)
     S = ns.image_size
@@ -151,13 +154,14 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; not measured here
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "data-sheet"
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
 def _reference_root():
     """The unmodified reference tree, when one is reachable on this box (it is not shipped to the GPU boxes)."""
-    for c in (os.environ.get("MCVD_REFERENCE_ROOT"), "/root/reference", os.path.join(ROOT, "baseline", "_ref")):
+    for c in (os.environ.get("MCVD_REFERENCE_ROOT"), os.path.join(ROOT, "oracle", "_ref")):
         if c and os.path.exists(os.path.join(c, "models", "better", "ncsnpp_more.py")):
             return c
     return None
@@ -364,12 +368,14 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = [None]
+
     def timed(fn, K):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(K):
-            fn(i)
+            last[0] = fn(i)
         e1.record()
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1)
@@ -390,6 +396,8 @@ def main():
     clocks.start()
     ms = timed(step_resident, args.steps)
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0])
     frames_per_step = n_clips * nfp
     value = frames_per_step * args.steps / (ms / 1e3)
     log(f"resident: {ms / args.steps:.1f} ms/step -> {value:.1f} frames/s")
@@ -410,13 +418,13 @@ def main():
     line = {
         "metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": args.scaling,
-        "vs_baseline": None, "dtype": "f32 (fp16 hi/lo split on tcgen05, fp32 accumulate)", "data": "synthetic",
+        "vs_baseline": None, "dtype": "f32 (fp16 hi/lo split on wgmma, fp32 accumulate)", "data": "synthetic",
         "config": {"workload": f"{args.workload}: {describe(cfg)}", "clips_per_gpu": B, "global_clips": n_clips,
                    "mode": (f"autoregressive video_gen: {n_iter} sampler calls per step, {nfp} frames kept of "
                             f"{F * n_iter} generated per clip" if args.ar else "one ddpm_sampler call per step"),
                    "parallelism": f"clip-sharded x{world} (distinct clips per rank, global clip ids), no data-path "
                                   f"collective; one NCCL all-gather of the finished frames inside the e2e region",
-                   "l2": "working set (weights 4x%.0f MB + GBs of activations per forward) exceeds the 126 MB L2; no flush needed"
+                   "l2": "working set (weights 4x%.0f MB + GBs of activations per forward) exceeds the 50 MB L2; no flush needed"
                          % (sum(p.numel() for p in net.parameters()) / 1e6),
                    "conv_backend": net.engine().conv_mode, "noise": "in-kernel Philox4x32-10 keyed by global clip id"},
         "e2e": {"value": e2e_val, "unit": "frames/s", "ms_per_step": ms_e2e / args.steps,
@@ -430,7 +438,7 @@ def main():
         "flops": {"algorithmic_gflop_per_sample_forward": gf,
                   "algorithmic_tflop_per_kept_frame": gf * calls / nfp / 1e3,
                   "whole_path_achieved_tflops": value * gf * calls / nfp / 1e3 / world,
-                  "whole_path_frac_of_bf16_peak": value * gf * calls / nfp / 1e3 / world / pk["bf16_tflops_sustained"],
+                  "whole_path_frac_of_bf16_peak": value * gf * calls / nfp / 1e3 / world / peak_tflops(pk),
                   "note": "tensor work executed = 3x algorithmic (fp16 hi/lo split for fp32 parity)"},
     }
 
@@ -454,9 +462,33 @@ def main():
         dist.destroy_process_group()
 
 
+DUMP_LIMIT = 64_000_000          # bytes of all files written, .npy headers included
+
+
+def peak_tflops(pk):
+    """the tensor rate fractions are taken against: a measured sustained rate when one is recorded, else the peak"""
+    return pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+
+
+def dump_outputs(path, frames):
+    """The frames [clips, C*frames, H, W] in [0, 1] that the last timed step returned on this process (rank 0: its
+    own clips when several GPUs run), as float32; when they exceed 64 MB a fixed-seed sample of whole clips (sorted
+    clip ids, stored in clip_ids.npy) is written instead, both files together within 64 MB."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    a = frames.detach().float().cpu().numpy()
+    per_clip = a[0].nbytes + 8                                    # frames + the clip's id
+    if a.nbytes + 128 > DUMP_LIMIT:
+        keep = np.sort(np.random.default_rng(0).choice(a.shape[0], (DUMP_LIMIT - 2 * 128) // per_clip, replace=False))
+        np.save(os.path.join(path, "clip_ids.npy"), keep.astype(np.int64).astype(np.float64))
+        a = a[keep]
+    np.save(os.path.join(path, "frames.npy"), np.ascontiguousarray(a, dtype=np.float32))
+    log(f"wrote {a.shape} float32 frames to {path}")
+
+
 def roofline(net, P, B, cfg, pk, pk_src):
     """Per-op CUDA-event timing of the lowered program (2 forwards after a warm-up one), on the launch
-    stream; the dominant kernel is the tcgen05 implicit-GEMM conv (k_conv_umma)."""
+    stream; the dominant kernel is the wgmma implicit-GEMM conv (k_conv_umma)."""
     from mcvd_b200 import lib
     eng = net.engine()
     n = len(P.step_ops)
@@ -491,8 +523,9 @@ def roofline(net, P, B, cfg, pk, pk_src):
     per_kind = {names[k][3:].lower(): {"ms_per_forward": v[0] / reps, "launches_per_forward": v[1] // reps}
                 for k, v in sorted(tot.items(), key=lambda kv: -kv[1][0])}
     total_ms = sum(v[0] for v in tot.values()) / reps
-    out = {"bound": "tensor", "unit": "TFLOP/s", "peak": pk["bf16_tflops_sustained"],
-           "peak_source": f"{pk_src} cuBLAS bf16 sustained (MEASURED_PEAKS.json)", "traffic": None,
+    out = {"bound": "tensor", "unit": "TFLOP/s", "peak": peak_tflops(pk),
+           "peak_source": ("measured cuBLAS bf16 sustained rate (MEASURED_PEAKS.json)" if pk_src == "measured"
+                           else "H100 SXM data-sheet dense bf16 peak (not a measured rate)"), "traffic": None,
            "per_kind": per_kind, "forward_ms_sum_of_kernels": total_ms}
     conv_kind = lib.OP_CONV_UMMA if lib.OP_CONV_UMMA in tot else lib.OP_CONV_UMMA2
     if conv_kind in tot:
@@ -515,10 +548,9 @@ def roofline(net, P, B, cfg, pk, pk_src):
         out["algorithmic_bytes_per_launch"] = alg_bytes / max(n_umma, 1)
         ms_umma = tot[conv_kind][0] / reps
         ach = flops_umma / (ms_umma / 1e3) / 1e12
-        out.update(kernel=("k_conv_umma (3x3) + k_conv1x1_umma (1x1)" if conv_kind == lib.OP_CONV_UMMA
-                           else "k_conv_umma2 (cta_group::2)") + " (tcgen05 implicit-GEMM convs, all conv launches of one forward)",
-                   achieved=ach, frac=ach / pk["bf16_tflops_sustained"], executed_tflops=3 * ach,
-                   executed_frac=3 * ach / pk["bf16_tflops_sustained"],
+        out.update(kernel="k_conv_umma (wgmma implicit-GEMM convs, all conv launches of one forward)",
+                   achieved=ach, frac=ach / peak_tflops(pk), executed_tflops=3 * ach,
+                   executed_frac=3 * ach / peak_tflops(pk),
                    kernel_share_of_forward=ms_umma / total_ms,
                    algorithmic_gflop_per_forward_in_kernel=flops_umma / 1e9)
     else:

@@ -1,5 +1,5 @@
 /*
- * mcvd_b200 -- C ABI of the B200-native MCVD DDPM-sampling hot path.
+ * mcvd_b200 -- C ABI of the H100-native (sm_90a) MCVD DDPM-sampling hot path.
  *
  * Plain C: device pointers and sizes only, no torch types.  Every pointer is a BORROWED device
  * pointer (owned by the caller, normally a torch tensor); outputs and workspaces are caller
@@ -13,7 +13,7 @@
  *     MCVD_F_UP / MCVD_F_DOWN (the FIR is fused with the norm/activation that precedes it);
  *   - everything else on the path is ATen/cuDNN/cuBLAS reached from Python
  *     (models/better/layerspp.py, layers.py, ncsnpp_more.py, models/__init__.py); the op kinds below
- *     are the fused B200 equivalents, each citing the reference lines it stands for.
+ *     are the fused H100 equivalents, each citing the reference lines it stands for.
  *
  * The host side (mcvd_b200/program.py) lowers a network + sampler step into an array of McvdOp and
  * calls mcvd_run_program() once per network evaluation (or once per CUDA-graph capture).
@@ -93,49 +93,48 @@ enum {
    * dst = x [B,C0,H,W] NCHW (in place); src0 = eps [B,H,W,C0] NHWC (channel pitch Cout if > 0); src1 = z NCHW or NULL
    * (MCVD_F_PHILOX: z from Philox4x32-10 keyed by (seed=i0|i1<<32, clip id = i2 + b, step = i3)). */
   MCVD_OP_DIFFUSION_UPDATE = 11,
-  /* 3x3 / 1x1 convolution on the 5th-gen tensor cores (tcgen05.mma kind::f16, fp16 hi/lo split of
-   * both operands, fp32 accumulation in TMEM), with the GroupNorm/FiLM/SiLU transform of the input
+  /* 3x3 / 1x1 convolution on the Hopper tensor cores (wgmma m64nNk16 f16, fp16 hi/lo split of
+   * both operands, fp32 accumulation in registers), with the GroupNorm/FiLM/SiLU transform of the input
    * fused into the shared-memory staging.  Same semantics as MCVD_OP_CONV_SIMT; see
-   * mcvd_b200/csrc/conv_umma.cu.  aux1 = norm table of (src0|src1) or NULL; i1 = n tile; i2 = accumulators
-   * per tile (0 = auto); i3 = operand split for accuracy experiments (0 | 3 = all three products, 1 = drop
+   * mcvd_b200/csrc/conv_umma.cu.  aux1 = norm table of (src0|src1) or NULL; i1 = n tile; i2 = work
+   * organisation: 1 = streaming (one 128-position x n-tile tile per work item), 2 = input-stationary (1x1 convs
+   * without a second segment: a 128-position tile's input stays resident in shared memory while the weights of
+   * every n tile stream past it; streaming where it does not fit), 0 = input-stationary where it applies and the
+   * position tiles fill the GPU, else streaming; i3 = operand split for accuracy experiments (0 | 3 = all three products, 1 = drop
    * hi*lo_w, 2 = drop lo_a*hi, 4 = hi*hi only); f1 = weight un-scale.  Optional second K-segment (src2|src3 with C2|C3 channels, RAW,
    * centre tap only, weights appended per n-tile): the 1x1 shortcut Conv_2(x) of ResnetBlockBigGANpp
-   * (layerspp.py:618-619) accumulated into the same TMEM tile as Conv_1, so
+   * (layerspp.py:618-619) accumulated into the same accumulators as Conv_1, so
    * dst = f0 * (Conv_1(act(norm(h))) + Conv_2(x) + bias + residual) in ONE kernel.
    * dst2 = NULL, or the int64 tile statistics of the stored output (format and meaning as in MCVD_OP_CONV_UMMA2:
    * [tiles][NJ][2][Cout], mcvd_umma2_stats_bytes() bytes) for the GroupNorm that reads dst next;
-   * aux2 = NULL or int64 [grid][16] cycle counters (tools/umma_timing.py).
-   * Kernel size 1 without a second segment and without dst2 (NIN / q,k,v / skip projections,
-   * layers.py:541-556, layerspp.py:230-249,618-619) is served by the input-stationary kernel of
-   * mcvd_b200/csrc/conv1x1_umma.cu (same weights, bit-identical results) when the channel counts are multiples
-   * of 32 and, with a norm table, the maps hold >= 64 positions; MCVD_CONV1X1=0 in the environment disables it. */
+   * aux2 is ignored. */
   MCVD_OP_CONV_UMMA = 12,
   /* final 3x3 conv with tiny Cout (<= 16) and fused input norm: conv3x3(SiLU(GN(x))) of
    * ncsnpp_more.py:375-379; aux0 = float4 norm table or NULL. */
   MCVD_OP_CONV_SMALLN = 13,
   /* dst[i] = src0[i] (i0 floats) -- device-to-device copy inside a program. */
   MCVD_OP_COPY = 14,
-  /* MCVD_OP_ATTENTION on the tensor cores (tcgen05, fp16 hi/lo split, flash-style online softmax with
-   * S and the per-tile P.V product in TMEM); same fields plus dst2 = device scratch of at least
+  /* MCVD_OP_ATTENTION on the tensor cores (wgmma, fp16 hi/lo split, flash-style online softmax with
+   * S and O in registers); same fields plus dst2 = device scratch of at least
    * mcvd_attention_scratch_bytes(B, H*W, C0) bytes (16-byte aligned): a first kernel splits q, k, v into
    * fp16 hi/lo operand images there, the attention kernel streams them in with cp.async.bulk (2 launches).
    * Head dim in {32,48,64,96,128,192}, H*W a multiple of the key tile (128; 64 for head dim 128; 32 for head
    * dim 192; H*W itself when smaller).  See mcvd_b200/csrc/attention_umma.cu. */
   MCVD_OP_ATTENTION_UMMA = 15,
-  /* MCVD_OP_CONV_UMMA on CTA pairs (tcgen05.mma.cta_group::2, M = 256 over the two SMs of a TPC; see
-   * mcvd_b200/csrc/conv_umma2.cu).  Same semantics and fields, except:
+  /* MCVD_OP_CONV_UMMA with the norm table in planar form (same wgmma kernel, mcvd_b200/csrc/conv_umma.cu).  Same
+   * semantics and fields, except:
    *   aux1 = norm table of (src0|src1) in the planar layout [B][3][C0+C1] = mean | rstd*G | S that
    *          MCVD_OP_GN_FINALIZE writes to its dst2 (NULL: raw input);
    *   w    = weights packed by mcvd_umma2_pack_weights for n tile i1 and K-block i2
    *          (i2 = mcvd_umma2_plan(...); 0 skips the consistency check);
    *   i3   = operand split: 3 (default, also 0) = hi*hi + lo*hi + hi*lo, 1 = drop hi*lo (fp16 weights),
-   *          2 = drop lo*hi (fp16 activations), 4 = hi*hi only -- accuracy experiments, DESIGN.md section 4;
+   *          2 = drop lo*hi (fp16 activations), 4 = hi*hi only -- accuracy experiments;
    *   dst2 = NULL, or int64 [tiles][NJ][2][Cout] receiving the GroupNorm partial sums of the stored output
    *          (sum and sum of squares of round(x * 2^16), exact integer arithmetic; tiles = 128-position row
    *          tiles of the padded-flat position space, NJ = 127 / Pimg + 2 image slots per tile,
    *          mcvd_umma2_stats_bytes() bytes) -- nn.GroupNorm statistics of the NEXT act-norm
    *          (layerspp.py:474-477) without re-reading the activation;
-   *   aux2 = NULL or int64 [grid][16] cycle counters (tools/umma_timing.py). */
+   *   aux2 is ignored. */
   MCVD_OP_CONV_UMMA2 = 16,
   /* per-frame quality metrics of generated clips on the GPU (reference runners/ncsn_runner.py:1581-1600, which
    * loops over PIL images on the CPU): src0 = pred, src1 = real, both [B, C0*i0, H, W] fp32 in [0,1] (i0 frames of
@@ -218,13 +217,13 @@ int mcvd_umma_kblock(int C0, int C1);
  * statistics (the shared-memory plan depends on all of them); the weights must be packed with this value. */
 int mcvd_umma2_plan(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats);
 /* The shared-memory plan behind mcvd_umma2_plan (diagnostics / tests; host arithmetic only): out[0..7] = K-block,
- * slab rows, image stages, raw-ring stages, weight stages, image slots per tile, TMEM columns, dynamic shared
+ * slab rows, image stages, raw-ring stages, weight stages, image slots per tile, 0, dynamic shared
  * memory bytes.  Returns 0, or -1 when the conv cannot run on this kernel. */
 int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats, int* out);
 /* Bytes of the dst2 statistics array of a MCVD_OP_CONV_UMMA2 op. */
 long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cout);
-/* Weight packing for MCVD_OP_CONV_UMMA2.  w_taps = fp32 [taps][Cin][Cout]; every (n tile, K-block, tap) becomes
- * two shared-memory images (one per CTA of the pair, NT/2 output columns each).  A conv with a fused 1x1
+/* Weight packing for MCVD_OP_CONV_UMMA2 (the MCVD_OP_CONV_UMMA layout).  w_taps = fp32 [taps][Cin][Cout]; every
+ * (n tile, K-block, tap) becomes one shared-memory image of the n tile's columns.  A conv with a fused 1x1
  * shortcut is packed with two calls into the same `out`: the main conv with stage_off = 0 and the shortcut
  * with stage_off = (Cin_main / KB) * taps, both with per_unit = total stages of one n tile.  Returns the bytes
  * this call fills (taps*Cin*Cout*4); out == NULL only queries. */

@@ -1,4 +1,4 @@
-"""mcvd_b200 -- B200-native (sm_100a) implementation of the MCVD DDPM-sampling hot path.
+"""mcvd_b200 -- H100-native (sm_90a) implementation of the MCVD DDPM-sampling hot path.
 
 Public surface mirrors the reference (voletiv/mcvd-pytorch): ``get_model(config)``,
 ``ddpm_sampler / ddim_sampler / FPNDM_sampler``, ``get_sampler(config)``, ``conditioning_fn`` and the

@@ -1,6 +1,6 @@
-"""Build the sm_100a C-ABI library ``mcvd_b200/_lib/libmcvd_b200.so`` in-tree with nvcc.
+"""Build the sm_90a (H100) C-ABI library ``mcvd_b200/_lib/libmcvd_b200.so`` in-tree with nvcc.
 
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` cross-compiles without a GPU; the .so is
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` cross-compiles without a GPU; the .so is
 git-ignored but travels to the GPU box with the repo snapshot.  Rebuilds only when a source is
 newer than the library.
 """
@@ -15,9 +15,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(LIBDIR, "libmcvd_b200.so")
-SOURCES = ["api.cu", "elementwise.cu", "conv_simt.cu", "conv_smalln.cu", "attention_simt.cu", "conv_umma.cu", "conv_umma2.cu", "conv1x1_umma.cu",
+SOURCES = ["api.cu", "elementwise.cu", "conv_simt.cu", "conv_smalln.cu", "attention_simt.cu", "conv_umma.cu",
            "attention_umma.cu"]
-HEADERS = [os.path.join(CSRC, "mcvd_common.cuh"), os.path.join(CSRC, "umma_ptx.cuh"), os.path.join(os.path.dirname(HERE), "include", "mcvd_b200.h")]
+HEADERS = [os.path.join(CSRC, "mcvd_common.cuh"), os.path.join(CSRC, "umma_ptx.cuh"), os.path.join(CSRC, "wgmma_ops.cuh"), os.path.join(os.path.dirname(HERE), "include", "mcvd_b200.h")]
 
 
 def _nvcc() -> str:
@@ -64,7 +64,7 @@ def _build_locked(force: bool, verbose: bool) -> str:
                 os.path.getmtime(p) for p in [src] + HEADERS):
             continue
         tmp = obj + f".tmp{os.getpid()}"
-        cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+        cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                "-Xcompiler", "-fPIC", "-Xptxas", "-v" if verbose else "-warn-spills", "-c", src, "-o", tmp]
         procs.append((src, tmp, obj, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     failed = None

@@ -3,9 +3,8 @@
 The reference drives everything from YAML files turned into nested ``argparse.Namespace``
 objects (reference ``main.py:359-367`` ``dict2namespace``) and read with
 ``getattr(config.model, name, default)`` all over the model code.  The GPU box has no copy of
-the reference, so the five BASELINE.json workloads are restated here programmatically with the
-same field names (values after the ``--config_mod`` overrides BASELINE.json implies, see
-SURVEY.md section 0 D4/D5).  ``namespace_from_dict`` is the equivalent of ``dict2namespace`` so a
+the reference, so the five benchmark workloads are restated here programmatically with the
+same field names (values after the ``--config_mod`` overrides the workloads imply).  ``namespace_from_dict`` is the equivalent of ``dict2namespace`` so a
 YAML loaded by the caller works as well.
 """
 from __future__ import annotations
@@ -66,7 +65,7 @@ def _mk(name, batch, data=None, model=None, sampling=None):
 
 
 def workload(name: str) -> argparse.Namespace:
-    """Return one of the BASELINE.json workloads (``cfg1`` .. ``cfg5``) or a small test config.
+    """Return one of the benchmark workloads (``cfg1`` .. ``cfg5``) or a small test config.
 
     cfg1  smmnist_DDPM_small5.yml + model.arch=unetmore, subsample=10, B=2
     cfg2  smmnist_DDPM_big5.yml   + ngf=96 n_head_channels=96, subsample=100, B=64   (the headline)

@@ -1,15 +1,15 @@
-// Multi-head self-attention over the H*W tokens of a sample on the tcgen05 tensor cores, flash style
+// Multi-head self-attention over the H*W tokens of a sample on the Hopper tensor cores (wgmma), flash style
 // (reference AttnBlockpp.forward, models/better/layerspp.py:239-245: w = softmax_j(q_i.k_j * Ch^-0.5),
 // h_i = sum_j w_ij v_j; the reference materialises w as [B*heads, HW, HW] fp32).
 //
 //   qkv [B, T, 3C] fp32 (q | k | v along channels; head h = channels [h*d, (h+1)*d)),  out [B, T, C]
 //   grid = (ceil(T / 128), heads, B); one CTA owns 128 query rows and walks the keys in tiles of KT.
 //
-// Per key tile:   S = Q K^T   (tcgen05.mma, M=128, N=KT, K=d)          -> TMEM columns [0, KT)
-//                 P = exp(S*scale - m)  by the softmax warps (query row = TMEM lane: no shuffles),
-//                     written to smem as the A operand of the next MMA
-//                 O_tile = P V (M=128, N=d, K=KT)                       -> TMEM columns [KT, KT+d)
-//                 o = o * exp(m_old - m_new) + O_tile   in registers
+// Per key tile, each of the two consumer warpgroups (64 query rows):
+//                 S = Q K^T   (wgmma m64nKTk16, both operands from shared memory)   -> registers
+//                 P = exp(S*scale - m), online max / sum in registers (a row lives in the 4 lanes of a quad)
+//                 O = O * exp(m_old - m_new) + P V   (wgmma m64nDk16, P from registers: the fp32 accumulator
+//                     layout of S is the register A-operand layout, so P never touches shared memory)
 // fp32 parity: q, k, v and p are split into fp16 hi + lo and every product is 3 MMAs
 // (hi*hi + lo*hi + hi*lo), fp32 accumulation -- same scheme as conv_umma.cu.
 //
@@ -18,15 +18,9 @@
 //
 // Two launches per op:
 //   k_attn_presplit  converts q, k, v ONCE into fp16 hi/lo "operand images" in a scratch buffer, one image per
-//                    (sample, head, tile), byte-for-byte what the MMA wants in shared memory.  (Converting
-//                    inside the attention kernel re-did the K/V tiles for each of the T/128 query tiles
-//                    and left it bound by the latency of the staging loops: 400 us at 32x32 in cfg2.)
+//                    (sample, head, tile), byte-for-byte what the MMA wants in shared memory (converting inside
+//                    the attention kernel would redo the K/V tiles for each of the T/128 query tiles).
 //   k_attention_umma one thread streams the images in with cp.async.bulk (mbarrier complete_tx).
-// Warps: 0-7 softmax / output: query row r <-> TMEM lane r is shared by TWO threads (warp w and w+4 both own
-//        lane group w%4, the only TMEM lanes either may touch); each takes half of the key columns of S and half of
-//        the channels of O, and they meet through shared memory for the row maximum and the final row sum.  (One
-//        thread per row left a single warp per SMSP running a dependent MUFU / tcgen05.ld chain: 29 % issue slots.)
-//        8 image loader, 9 TMEM allocation + MMA issue.
 #include "mcvd_common.cuh"
 #include "umma_ptx.cuh"
 
@@ -37,8 +31,7 @@ namespace {
 using namespace ptx;
 
 constexpr int QT = 128;
-constexpr int ATT_THREADS = 320;       // 8 softmax warps + image loader + MMA issuer
-constexpr int SOFTMAX_THREADS = 256;
+constexpr int ATT_THREADS = 288;       // 2 consumer warpgroups + image loader
 constexpr int SPLIT_THREADS = 256;
 
 struct AttnArgs {
@@ -46,7 +39,7 @@ struct AttnArgs {
   float* out;
   uint8_t* img;                 // operand images: [Q tiles | K tiles | V tiles], see image_offsets()
   long long k_off, v_off;       // byte offsets of the K and V image arrays
-  int T, C, KT, nkt, nqt, tmem_cols;
+  int T, C, KT, nkt, nqt, nst;
   float scale;
 };
 
@@ -133,6 +126,9 @@ __device__ __forceinline__ void stage_v(uint8_t* vh, uint8_t* vl, const float* v
   }
 }
 
+// key tile: as large as the operand images allow in shared memory (Q is resident: 4*D*128 bytes)
+template <int D> __host__ __device__ constexpr int kt_max() { return D <= 96 ? 128 : (D <= 128 ? 64 : 32); }
+
 // image sizes in bytes (hi plane + lo plane)
 template <int D> __host__ __device__ constexpr long long q_image_bytes() { return 2LL * (D / 8) * QT * 16; }
 template <int D> __host__ __device__ inline long long kv_image_bytes(int KT) { return 2LL * (D / 8) * KT * 16; }
@@ -162,185 +158,174 @@ __global__ void __launch_bounds__(SPLIT_THREADS) k_attn_presplit(const AttnArgs 
   }
 }
 
-template <int D>
+// Attention kernel: grid (nqt, heads, B), 288 threads.  Warps 0-7 = two consumer warpgroups (query rows
+// [64 wg, 64 wg + 64) of the tile), warp 8 = image loader (Q once, then K / V^T tiles through NST stages).
+template <int D, int KT>
 __global__ void __launch_bounds__(ATT_THREADS, 1) k_attention_umma(const AttnArgs a) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  const int KT = a.KT;
-  const uint32_t q_half = (D / 8) * QT * 16, k_half = (D / 8) * KT * 16, v_half = (KT / 8) * D * 16,
-                 p_half = (KT / 8) * QT * 16;
-  uint8_t* qh = smem_raw;           uint8_t* ql = qh + q_half;
-  uint8_t* kh = ql + q_half;        uint8_t* kl = kh + k_half;
-  uint8_t* vh = kl + k_half;        uint8_t* vl = vh + v_half;
-  uint8_t* ph = vl + v_half;        uint8_t* pl = ph + p_half;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(pl + p_half);
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  constexpr int NQ = QT / 64;                 // consumer warpgroups
+  const int NST = a.nst;
+  const uint32_t q_bytes = (uint32_t)q_image_bytes<D>(), kv_bytes = (uint32_t)kv_image_bytes<D>(KT);
+  uint8_t* qimg = smem_raw;                   // hi | lo
+  uint8_t* kimg = qimg + q_bytes;             // [NST] hi | lo
+  uint8_t* vimg = kimg + (size_t)NST * kv_bytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(vimg + (size_t)NST * kv_bytes);
   const uint32_t bar0 = smem_u32(bars);
-  const uint32_t K_FULL = bar0, V_FULL = bar0 + 8, P_FULL = bar0 + 16, S_FULL = bar0 + 24, O_FULL = bar0 + 32;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
-  float* xmax = reinterpret_cast<float*>(bars + 8);        // [tile parity][half][QT] partial row maxima
-  float* xsum = xmax + 4 * QT;                             // [half][QT] partial row sums
+  const uint32_t Q_FULL = bar0;
+  auto K_FULL = [&](int i) { return bar0 + 8u * (1 + i); };
+  auto V_FULL = [&](int i) { return bar0 + 8u * (3 + i); };
+  auto K_EMPTY = [&](int i) { return bar0 + 8u * (5 + i); };
+  auto V_EMPTY = [&](int i) { return bar0 + 8u * (7 + i); };
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int q0 = blockIdx.x * QT, h = blockIdx.y, b = blockIdx.z;
   const long long bh = (long long)b * gridDim.y + h;
 
   if (tid == 0) {
-    mbar_init(K_FULL, 1); mbar_init(V_FULL, 1); mbar_init(P_FULL, SOFTMAX_THREADS);
-    mbar_init(S_FULL, 1); mbar_init(O_FULL, 1);
+    mbar_init(Q_FULL, 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(K_FULL(i), 1); mbar_init(V_FULL(i), 1);
+      mbar_init(K_EMPTY(i), 4 * NQ); mbar_init(V_EMPTY(i), 4 * NQ);
+    }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc(smem_u32(tmem_slot), (uint32_t)a.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tO = tmem_base + (uint32_t)KT;
 
-  if (warp < 8) {
-    // ================= softmax + output accumulation: two threads per query row =================
-    const int lg = warp & 3, hf = warp >> 2;                // TMEM lane group, column / channel half
-    const int r = lg * 32 + (tid & 31);
-    const uint32_t lane_off = (uint32_t)(lg * 32) << 16;
-    constexpr int D0 = ((D / 2 + 15) / 16) * 16;            // channels of half 0 (half 1 takes the rest)
-    const int oc0 = hf ? D0 : 0, n_o = hf ? D - D0 : D0;
-    const int half_cols = KT / 2;                           // 64 or 32 key columns per thread and tile
-    const int col0 = hf * half_cols;
-    float o[D0];
-#pragma unroll
-    for (int i = 0; i < D0; ++i) o[i] = 0.f;
-    float m = -INFINITY, l = 0.f;                           // l: this thread's share of the row sum
-    for (int j = 0; j < a.nkt; ++j) {
-      mbar_wait(S_FULL, j & 1);
-      tc_fence_after();
-      // this thread's columns of S(j): read once, kept in registers across the max exchange
-      uint32_t rr[64];                                      // half_cols = 16 (head dim 192), 32 or 64 of them are live
-      tmem_ld16(tS + lane_off + col0, rr);
-      if (half_cols >= 32) tmem_ld16(tS + lane_off + col0 + 16, rr + 16);
-      if (half_cols == 64) {
-        tmem_ld16(tS + lane_off + col0 + 32, rr + 32);
-        tmem_ld16(tS + lane_off + col0 + 48, rr + 48);
+  if (warp == 4 * NQ) {
+    // ================= image loader =================
+    if (elect_one()) {
+      mbar_arrive_expect_tx(Q_FULL, q_bytes);
+      bulk_g2s(smem_u32(qimg), a.img + (bh * a.nqt + blockIdx.x) * q_image_bytes<D>(), q_bytes, Q_FULL);
+      for (int kt = 0; kt < a.nkt; ++kt) {
+        const int st = kt % NST;
+        const uint32_t ph = ((kt / NST) & 1) ^ 1;
+        const long long off = (bh * a.nkt + kt) * kv_image_bytes<D>(KT);
+        mbar_wait(K_EMPTY(st), ph);
+        mbar_arrive_expect_tx(K_FULL(st), kv_bytes);
+        bulk_g2s(smem_u32(kimg + (size_t)st * kv_bytes), a.img + a.k_off + off, kv_bytes, K_FULL(st));
+        mbar_wait(V_EMPTY(st), ph);
+        mbar_arrive_expect_tx(V_FULL(st), kv_bytes);
+        bulk_g2s(smem_u32(vimg + (size_t)st * kv_bytes), a.img + a.v_off + off, kv_bytes, V_FULL(st));
       }
-      tmem_ld_wait();
+    }
+    __syncwarp();
+    return;
+  }
+
+  // ================= consumers: S = Q K^T, online softmax, O += P V =================
+  const int wg = warp >> 2, wq = warp & 3;
+  const int r0 = 64 * wg + 16 * wq + (lane >> 2);          // query rows r0 and r0 + 8 of the tile
+  const int cq = 2 * (lane & 3);
+  // descriptors: Q rows at 16 B, K-chunks QT*16 apart; K tile rows (keys) at 16 B, chunks KT*16 apart;
+  // V^T rows (channels) at 16 B, key chunks D*16 apart
+  const uint64_t q_desc = make_desc(smem_u32(qimg) + 64u * 16u * wg, QT * 16, 128);
+  const uint32_t q_lo16 = q_bytes / 32;                      // lo plane offset, 16-byte units
+  const uint32_t kv_lo16 = kv_bytes / 32;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  mbar_wait(Q_FULL, 0);
+  for (int kt = 0; kt < a.nkt; ++kt) {
+    const int st = kt % NST;
+    const uint32_t ph = (kt / NST) & 1;
+    float sacc[KT / 2];
+    const uint64_t k_desc = make_desc(smem_u32(kimg + (size_t)st * kv_bytes), KT * 16, 128);
+    mbar_wait(K_FULL(st), ph);
+    wgmma_fence();
+#pragma unroll
+    for (int s = 0; s < D / 16; ++s) {
+      const uint64_t qh = desc_add(q_desc, 2u * s * QT), ql = desc_add(qh, q_lo16);
+      const uint64_t kh = desc_add(k_desc, 2u * s * KT), kl = desc_add(kh, kv_lo16);
+      wgmma_ss<KT>(sacc, qh, kh, s);
+      wgmma_ss<KT>(sacc, ql, kh, 1);
+      wgmma_ss<KT>(sacc, qh, kl, 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < KT / 2; ++i) reg_fence(sacc[i]);
+    if (lane == 0) mbar_arrive(K_EMPTY(st));
+    // online softmax: a query row lives in the 4 lanes of a quad
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
       float mx = -INFINITY;
 #pragma unroll
-      for (int e = 0; e < 16; ++e) mx = fmaxf(mx, __uint_as_float(rr[e]));
-      if (half_cols >= 32) {
-#pragma unroll
-        for (int e = 16; e < 32; ++e) mx = fmaxf(mx, __uint_as_float(rr[e]));
-      }
-      if (half_cols == 64) {
-#pragma unroll
-        for (int e = 32; e < 64; ++e) mx = fmaxf(mx, __uint_as_float(rr[e]));
-      }
-      float* xm = xmax + (j & 1) * 2 * QT;                  // double-buffered by tile parity
-      xm[hf * QT + r] = mx;
-      named_bar_sync(1, SOFTMAX_THREADS);
-      mx = fmaxf(mx, xm[(hf ^ 1) * QT + r]);
-      // scale > 0, so max(s)*scale == max(s*scale)
-      const float mnew = fmaxf(m, mx * a.scale);
-      const float corr = __expf(m - mnew);
+      for (int j = 0; j < KT / 8; ++j)
+        mx = fmaxf(mx, fmaxf(sacc[4 * j + 2 * i], sacc[4 * j + 2 * i + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mn = fmaxf(m[i], mx * a.scale);
+      alpha[i] = expf(m[i] - mn);
+      m[i] = mn;
       float sum = 0.f;
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        if (g * 8 < half_cols) {
-          float p[8];
+      for (int j = 0; j < KT / 8; ++j) {
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            p[e] = __expf(fmaf(__uint_as_float(rr[g * 8 + e]), a.scale, -mnew));
-            sum += p[e];
-          }
-          uint4 hv, lv;
-          split8(p, hv, lv);
-          const size_t off = ((size_t)(col0 / 8 + g) * QT + r) * 16;
-          *reinterpret_cast<uint4*>(ph + off) = hv;
-          *reinterpret_cast<uint4*>(pl + off) = lv;
+        for (int e = 0; e < 2; ++e) {
+          const float p = expf(fmaf(sacc[4 * j + 2 * i + e], a.scale, -mn));
+          sacc[4 * j + 2 * i + e] = p;
+          sum += p;
         }
       }
-      l = l * corr + sum;
-      m = mnew;
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(P_FULL);
-      mbar_wait(O_FULL, j & 1);
-      tc_fence_after();
-      {
-        uint32_t ro[D0];
+      l[i] = l[i] * alpha[i] + sum;
+    }
 #pragma unroll
-        for (int c = 0; c < D0 / 16; ++c)
-          if (c * 16 < n_o) tmem_ld16(tO + lane_off + oc0 + c * 16, ro + c * 16);     // warp-uniform predicate
-        tmem_ld_wait();
+    for (int j = 0; j < D / 8; ++j) {
+      o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
+      o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+    }
+    // P (fp16 hi / lo pairs in the accumulator layout == the register A-operand layout of m64nNk16)
+    const uint64_t v_desc = make_desc(smem_u32(vimg + (size_t)st * kv_bytes), D * 16, 128);
+    mbar_wait(V_FULL(st), ph);
+    uint32_t ph4[KT / 16][4], pl4[KT / 16][4];
 #pragma unroll
-        for (int e = 0; e < D0; ++e)
-          if (e < n_o) o[e] = fmaf(o[e], corr, __uint_as_float(ro[e]));
-      }
-    }
-    tc_fence_before();
-    // row sum = the two halves' shares (same running maximum, so they simply add)
-    xsum[hf * QT + r] = l;
-    named_bar_sync(1, SOFTMAX_THREADS);
-    if (q0 + r < a.T) {
-      const float inv = 1.0f / (xsum[r] + xsum[QT + r]);
-      float* op = a.out + ((long long)b * a.T + q0 + r) * a.C + h * D + oc0;
+    for (int kk = 0; kk < KT / 16; ++kk)
 #pragma unroll
-      for (int c = 0; c < D0; c += 4)
-        if (c < n_o)
-          *reinterpret_cast<float4*>(op + c) = make_float4(o[c] * inv, o[c + 1] * inv, o[c + 2] * inv, o[c + 3] * inv);
+      for (int r = 0; r < 4; ++r) split2(sacc[8 * kk + 2 * r], sacc[8 * kk + 2 * r + 1], ph4[kk][r], pl4[kk][r]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < KT / 16; ++kk) {
+      const uint64_t vh = desc_add(v_desc, 2u * kk * D), vl = desc_add(vh, kv_lo16);
+      wgmma_rs<D>(o, ph4[kk], vh);
+      wgmma_rs<D>(o, pl4[kk], vh);
+      wgmma_rs<D>(o, ph4[kk], vl);
     }
-  } else if (warp == 8) {
-    // ================= image loader: one thread, cp.async.bulk global -> smem =================
-    if (elect_one()) {
-      const uint32_t qbytes = (uint32_t)q_image_bytes<D>(), kvbytes = (uint32_t)kv_image_bytes<D>(KT);
-      const uint8_t* qimg = a.img + (bh * a.nqt + blockIdx.x) * q_image_bytes<D>();
-      const uint8_t* kimg = a.img + a.k_off + bh * a.nkt * kv_image_bytes<D>(KT);
-      const uint8_t* vimg = a.img + a.v_off + bh * a.nkt * kv_image_bytes<D>(KT);
-      for (int j = 0; j < a.nkt; ++j) {
-        if (j > 0) mbar_wait(S_FULL, (j - 1) & 1);          // S_{j-1} done: K buffer free
-        // the Q image rides on the first K phase (q | k buffers are adjacent but filled by two copies)
-        mbar_arrive_expect_tx(K_FULL, kvbytes + (j == 0 ? qbytes : 0u));
-        if (j == 0) bulk_g2s(smem_u32(qh), qimg, qbytes, K_FULL);
-        bulk_g2s(smem_u32(kh), kimg + (long long)j * kvbytes, kvbytes, K_FULL);
-        if (j > 0) mbar_wait(O_FULL, (j - 1) & 1);          // PV_{j-1} done: V buffer free
-        mbar_arrive_expect_tx(V_FULL, kvbytes);
-        bulk_g2s(smem_u32(vh), vimg + (long long)j * kvbytes, kvbytes, V_FULL);
-      }
-    }
-  } else if (elect_one()) {
-    // ================= MMA issuer (one elected lane of warp 9) =================
-    const uint32_t idesc_s = make_idesc_f16(QT, KT), idesc_o = make_idesc_f16(QT, D);
-    const uint32_t q_lbo = QT * 16, k_lbo = (uint32_t)KT * 16, v_lbo = D * 16, p_lbo = QT * 16;
-    const uint32_t sqh = smem_u32(qh), sql = smem_u32(ql), skh = smem_u32(kh), skl = smem_u32(kl);
-    const uint32_t svh = smem_u32(vh), svl = smem_u32(vl), sph = smem_u32(ph), spl = smem_u32(pl);
-    for (int j = 0; j < a.nkt; ++j) {
-      mbar_wait(K_FULL, j & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int ks = 0; ks < D / 16; ++ks) {
-        const uint64_t dqh = make_desc(sqh + 2 * ks * q_lbo, q_lbo, 128), dql = make_desc(sql + 2 * ks * q_lbo, q_lbo, 128);
-        const uint64_t dkh = make_desc(skh + 2 * ks * k_lbo, k_lbo, 128), dkl = make_desc(skl + 2 * ks * k_lbo, k_lbo, 128);
-        umma_f16(tS, dqh, dkh, idesc_s, ks > 0 ? 1u : 0u);
-        umma_f16(tS, dql, dkh, idesc_s, 1u);
-        umma_f16(tS, dqh, dkl, idesc_s, 1u);
-      }
-      umma_commit(S_FULL);
-      mbar_wait(V_FULL, j & 1);
-      mbar_wait(P_FULL, j & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int ks = 0; ks < KT / 16; ++ks) {
-        const uint64_t dph = make_desc(sph + 2 * ks * p_lbo, p_lbo, 128), dpl = make_desc(spl + 2 * ks * p_lbo, p_lbo, 128);
-        const uint64_t dvh = make_desc(svh + 2 * ks * v_lbo, v_lbo, 128), dvl = make_desc(svl + 2 * ks * v_lbo, v_lbo, 128);
-        umma_f16(tO, dph, dvh, idesc_o, ks > 0 ? 1u : 0u);
-        umma_f16(tO, dpl, dvh, idesc_o, 1u);
-        umma_f16(tO, dph, dvl, idesc_o, 1u);
-      }
-      umma_commit(O_FULL);
-    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) reg_fence(o[i]);
+    if (lane == 0) mbar_arrive(V_EMPTY(st));
   }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int q = q0 + r0 + 8 * i;
+    if (q >= a.T) continue;
+    const float inv = 1.0f / l[i];
+    float* orow = a.out + ((long long)b * a.T + q) * a.C + h * D;
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j)
+      *reinterpret_cast<float2*>(orow + 8 * j + cq) = make_float2(o[4 * j + 2 * i] * inv, o[4 * j + 2 * i + 1] * inv);
+  }
+}
 
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
-  }
+template <int D, int KT>
+int launch_dk(const AttnArgs& a, size_t smem, const McvdOp& op, cudaStream_t s) {
+  cudaError_t e = cudaFuncSetAttribute(k_attention_umma<D, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  MCVD_CHECK(e == cudaSuccess, "ATTENTION_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+  dim3 sgrid(a.nqt + 2 * a.nkt, op.i0, op.B);
+  k_attn_presplit<D><<<sgrid, SPLIT_THREADS, 0, s>>>(a);
+  MCVD_CUDA_LAUNCH_CHECK("attention presplit");
+  dim3 grid(a.nqt, op.i0, op.B);
+  k_attention_umma<D, KT><<<grid, ATT_THREADS, smem, s>>>(a);
+  MCVD_CUDA_LAUNCH_CHECK("attention_umma");
+  return 0;
 }
 
 template <int D>
@@ -348,16 +333,11 @@ int launch_d(const McvdOp& op, cudaStream_t s) {
   AttnArgs a;
   a.qkv = (const float*)op.src0; a.out = (float*)op.dst;
   a.T = op.H * op.W; a.C = op.C0; a.scale = op.f0;
-  // key tile: as large as the operand images allow in 227 KB (Q is resident: 4*D*128 bytes; K, V^T, P scale with KT)
-  a.KT = (D <= 96) ? 128 : (D <= 128 ? 64 : 32);
+  a.KT = kt_max<D>();
   if (a.T < a.KT) a.KT = a.T;
-  // two softmax threads per query row split the key columns of a tile: 16, 32 or 64 columns each
   MCVD_CHECK((a.KT == 32 || a.KT == 64 || a.KT == 128) && a.T % a.KT == 0,
              "ATTENTION_UMMA: %d tokens not tileable by the key tile %d", a.T, a.KT);
   a.nkt = a.T / a.KT;
-  int cols = a.KT + D, p2 = 32;
-  while (p2 < cols) p2 <<= 1;
-  a.tmem_cols = p2;
   a.nqt = cdiv(a.T, QT);
   a.img = (uint8_t*)op.dst2;
   const long long bh = (long long)op.B * op.i0;
@@ -365,18 +345,15 @@ int launch_d(const McvdOp& op, cudaStream_t s) {
   a.v_off = a.k_off + bh * a.nkt * kv_image_bytes<D>(a.KT);
   MCVD_CHECK(op.dst2, "ATTENTION_UMMA: dst2 (operand-image scratch, mcvd_attention_scratch_bytes) is NULL");
   MCVD_CHECK((reinterpret_cast<uintptr_t>(op.dst2) & 15) == 0, "ATTENTION_UMMA: scratch must be 16-byte aligned");
-  const size_t smem = 2 * ((size_t)(D / 8) * QT * 16 + (size_t)(D / 8) * a.KT * 16 + (size_t)(a.KT / 8) * D * 16 +
-                           (size_t)(a.KT / 8) * QT * 16) + 64 + 6 * QT * sizeof(float);
+  // Q stays resident; K and V^T tiles are double-buffered when two stages fit
+  const size_t q_bytes = (size_t)q_image_bytes<D>(), kv_bytes = (size_t)kv_image_bytes<D>(a.KT);
+  a.nst = (q_bytes + 4 * kv_bytes + 128 <= 227 * 1024) ? 2 : 1;
+  const size_t smem = q_bytes + 2 * a.nst * kv_bytes + 128;
   MCVD_CHECK(smem <= 227 * 1024, "ATTENTION_UMMA: %zu B of shared memory", smem);
-  cudaError_t e = cudaFuncSetAttribute(k_attention_umma<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  MCVD_CHECK(e == cudaSuccess, "ATTENTION_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-  dim3 sgrid(a.nqt + 2 * a.nkt, op.i0, op.B);
-  k_attn_presplit<D><<<sgrid, SPLIT_THREADS, 0, s>>>(a);
-  MCVD_CUDA_LAUNCH_CHECK("attention presplit");
-  dim3 grid(a.nqt, op.i0, op.B);
-  k_attention_umma<D><<<grid, ATT_THREADS, smem, s>>>(a);
-  MCVD_CUDA_LAUNCH_CHECK("attention_umma");
-  return 0;
+  // key tiles never exceed kt_max<D>() (the S registers and shared memory are sized for it)
+  if (a.KT == 32) return launch_dk<D, 32>(a, smem, op, s);
+  if (a.KT == 64) return launch_dk<D, (kt_max<D>() >= 64 ? 64 : 32)>(a, smem, op, s);
+  return launch_dk<D, kt_max<D>()>(a, smem, op, s);
 }
 
 }  // namespace

@@ -1,12 +1,13 @@
-// 3x3 (pad 1) / 1x1 convolution on the Blackwell 5th-gen tensor cores (tcgen05.mma, accumulators in
-// TMEM), with the GroupNorm / FiLM / SiLU input transform fused into the shared-memory staging.
+// 3x3 (pad 1) / 1x1 convolution on the Hopper tensor cores (wgmma, fp32 accumulators in registers), with the
+// GroupNorm / FiLM / SiLU input transform fused into the shared-memory staging.  Serves MCVD_OP_CONV_UMMA and
+// MCVD_OP_CONV_UMMA2 (same kernel; the second reads the planar norm table and always pads the tile count to pairs).
 //
 // Reference semantics: nn.Conv2d 3x3 / 1x1 and NIN of models/better/layers.py:89-113,541-544 applied
 // to get_act_norm's output (layerspp.py:518-549), i.e. Conv_0 / Conv_1 / Conv_2 / NIN_* of
 // ResnetBlockBigGANppGN (layerspp.py:595-624) and AttnBlockpp (:230-249).
 //
 // fp32 parity on fp16 tensor cores: both operands are split  v = hi + lo  (hi = fp16(v),
-// lo = fp16(v - hi)) and three MMAs  hi*hi + lo*hi + hi*lo  accumulate in fp32 (TMEM); the dropped
+// lo = fp16(v - hi)) and three MMAs  hi*hi + lo*hi + hi*lo  accumulate in fp32; the dropped
 // lo*lo term and the second-level rounding are ~2^-22 relative.  Weights are pre-scaled by a power of
 // two (undone in the epilogue) so their lo parts stay in the fp16 normal range.
 //
@@ -14,31 +15,20 @@
 //     q = b*(H+1)*(W+1) + r*(W+1) + c,   r in [0,H], c in [0,W],   pixel (y,x) = (r-1, c-1)
 // where row r = 0 and column c = 0 are zero padding shared between neighbouring rows / images.  In
 // this indexing every 3x3 tap is a CONSTANT flat offset  dy*(W+1) + dx,  so a CTA stages ONE halo
-// slab [tile + 2*(W+1) + 2 positions] x [32 channels] of the transformed input in shared memory per
+// slab [tile + 2*(W+1) + 2 positions] x [KB channels] of the transformed input in shared memory per
 // K-block and all nine taps are shifted views of it: the A-operand descriptor of tap (dy,dx) is the
 // slab descriptor advanced by (dy*(W+1)+dx) * 16 bytes.  That needs a layout whose M-stride is 16
 // bytes, which is exactly the canonical no-swizzle K-major core-matrix layout
 //     [k-chunk of 8 halfs][position][8 halfs = 16 B]      LBO = positions*16 B,  SBO = 128 B.
 // Outputs at padding positions are computed and discarded (2..20 % of the rows).
 //
-// Round 2 (measurements in profiles/r2_*):
-//   * a second MMA-issuing warp (one per accumulator: a single thread's instruction stream, ~8 instructions per MMA at
-//     ~7 cycles each, was as slow as the tensor core itself);
-//   * row-per-lane epilogue: a lane owns one output position and writes its columns with 256-bit stores, the residual
-//     rows of the tile are prefetched into L2 while the accumulators are still pending; the shared-memory transpose
-//     remains only for the optional tile statistics;
-//   * optional GroupNorm partial sums of the stored output in exact 64-bit fixed point from the epilogue (op.dst2;
-//     same format and rationale as conv_umma2.cu; off by default, DESIGN.md section 3);
-//   * two producer threads per row on 128-row slabs, centre-rows-only staging of the fused-shortcut K-blocks;
-//   * plain 1x1 convolutions are handed to the input-stationary kernel of conv1x1_umma.cu by launch_conv_umma.
-//
-// Warp roles (480 threads, one CTA per SM):
-//   warps 0-7   producers: fp32 NHWC global -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab
+// Warp roles (384 threads, one CTA per SM, persistent over 128-position x NT tiles):
+//   warps 0-2   producers: fp32 NHWC global -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2 stages)
 //               (generic-proxy stores + fence.proxy.async)
-//   warp  8     weight loader: cp.async.bulk (TMA 1-D) of pre-packed fp16 hi/lo smem images
-//   warp  9     TMEM allocation + tcgen05.mma issue for accumulator 0, tcgen05.commit -> mbarriers
-//   warps 10-13 epilogue (TMEM lane quadrants 2,3,0,1): TMEM -> registers -> bias / residual / scale -> global
-//   warp  14    tcgen05.mma issue for accumulator 1 of two-accumulator tiles
+//   warp  3     weight loader: cp.async.bulk (TMA 1-D) of pre-packed fp16 hi/lo smem images (ring of NB stages)
+//   warps 4-11  two consumer warpgroups, 64 rows of the tile each: wgmma m64nNTk16 from the slab and weight
+//               stages, then the epilogue straight from the accumulator registers (bias / residual / scale /
+//               SiLU, optional GroupNorm statistics of the stored output)
 #include <cuda_fp16.h>
 
 #include "mcvd_common.cuh"
@@ -46,21 +36,22 @@
 
 namespace mcvd {
 
+constexpr int MT = 128;         // positions per tile (two consumer warpgroups x 64)
+
 namespace {
 
 using namespace ptx;
 
-constexpr int NPROD = 256;      // producer threads (warps 0-7)
-constexpr int W_LOAD = 8;       // weight-loader warp
-constexpr int W_MMA = 9;        // TMEM owner + MMA issuer warp
-constexpr int W_EPI = 10;       // first of the 4 epilogue warps (10..13 -> TMEM lane quadrants 2,3,0,1)
-constexpr int W_MMA2 = 14;      // second MMA issuer (accumulator 1 of two-accumulator tiles)
-constexpr int NTHREADS = 480;
+constexpr int NPROD = 96;       // producer threads (warps 0-2)
+constexpr int W_LOAD = 3;       // weight-loader warp
+constexpr int W_CONS = 4;       // first consumer warp (warpgroups 1 and 2)
+constexpr int NTHREADS = 384;   // 168 registers per thread: room for the 128 accumulators of NT = 256
 constexpr float STAT_SCALE = 65536.0f;   // fixed-point scale of the epilogue statistics
-constexpr int MT = 128;         // rows per accumulator (UMMA M)
 constexpr int TAB_NB = 8;       // images whose norm-table rows are staged in smem per K-block
+constexpr int HP_MAX = 512;
+constexpr int MAX_RESIDENT = 12;   // K-blocks an input-stationary work item keeps resident (12 x 8 KB at KB = 32)
 
-struct UmmaArgs {
+struct ConvArgs {
   const float* s0;
   const float* s1;
   const float* s2;       // second K-segment (fused 1x1 shortcut): raw sources, centre tap only
@@ -69,31 +60,31 @@ struct UmmaArgs {
   const __half* wpk;     // packed weights (see k_pack_weights)
   const float* bias;
   const float* res;
-  const float4* tab;     // norm table [B][Cin] (mean, rstd, G, S) or null
+  const float* tab;      // norm table or null: [B][Cin] float4 (mean, rstd, G, S), or planar [B][3][Cin]
+  int tab_planar;        //   (mean | rstd*G | S) when tab_planar
   float* dst;
   unsigned long long* stats;   // optional: [tiles128][NJ][2][Cout] fixed-point sum / sum of squares of the stored output
   int NJ;                // image slots per 128-position tile (127 / Pimg + 2)
-  long long* dbg;        // optional per-CTA cycle counters (tools/umma_timing.py); null in production
   int B, H, W, C0, C1, Cout;
   int ks;                // 1 or 3
   int Wp, Pimg;          // padded row pitch, positions per image
   long long Qtot;        // total flat positions
-  int NT, NACC, KB;      // n tile, accumulators per tile, channels per K-block (16|32)
+  int KB;                // channels per K-block (16|32)
   int HP;                // halo slab positions (multiple of 8)
   int halo0;             // slab index of the tile's first output position
   int nKB;               // K-blocks
   int NB;                // weight ring stages
-  int nsets;             // TMEM accumulator sets (2: epilogue of tile i overlaps the MMAs of tile i+1)
-  int tiles_n, ntiles;   // n tiles per m tile, total tiles
-  int tmem_cols;
+  int SA;                // slab stages: 2 (streaming), or nKB (input-stationary: the m tile's whole input resident)
+  int NPI;               // n tiles per work item: 1 (streaming) or tiles_n (input-stationary)
+  int tiles_n, ntiles;   // n tiles per m tile, work items
   int act_in, act_out;
-  int split;             // operand split (accuracy experiments, DESIGN.md section 4): bit 0 = lo*hi term, bit 1 = hi*lo term
+  int split;             // operand split (accuracy experiments): bit 0 = lo*hi term, bit 1 = hi*lo term
   int tab_nb;            // images a tile's slab can touch
   float wscale, oscale;
 };
 
 // position decode: flat q -> pixel index (b*H + y)*W + x, or -1 for padding / out of range
-__device__ __forceinline__ int decode_pos(const UmmaArgs& a, long long q, int& b_out) {
+__device__ __forceinline__ int decode_pos(const ConvArgs& a, long long q, int& b_out) {
   if (q < 0 || q >= a.Qtot) return -1;
   const int b = (int)(q / a.Pimg);
   const int r = (int)(q - (long long)b * a.Pimg);
@@ -106,221 +97,125 @@ __device__ __forceinline__ int decode_pos(const UmmaArgs& a, long long q, int& b
   return (b * a.H + rr) * a.W + cc;
 }
 
-// ---- the kernel: persistent CTAs, all phases overlapped ----------------------------------------------
-//   warps 0-7   producers : fp32 NHWC global -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2 stages)
-//   warp  8     loader    : cp.async.bulk of the pre-packed fp16 hi/lo weight images (ring of NB stages)
-//   warps 9,14  MMA       : TMEM allocation (9), one tcgen05.mma-issuing thread per accumulator, commits -> mbarriers
-//   warps 10-13 epilogue  : TMEM -> registers -> row-per-lane 256-bit global stores (smem transpose with statistics)
-// A CTA walks tiles blockIdx.x, +gridDim.x, ...; the A/B pipelines run across tile boundaries and the
-// accumulator is double-buffered in TMEM (when 2 * NACC * NT <= 512), so the producers of tile i+1, the
-// MMAs of tile i+1 and the epilogue of tile i all run concurrently, and CTAs drift out of lock-step.
-__global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const UmmaArgs a) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
+template <int NT>
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int chunks = a.KB / 8;
   const uint32_t a_half_bytes = (uint32_t)chunks * a.HP * 16;       // one of hi / lo
   const uint32_t a_stage_bytes = 2 * a_half_bytes;
-  const uint32_t b_step_bytes = 64u * a.NT;                          // one k16 step: hi (2 chunks) + lo
+  constexpr uint32_t b_step_bytes = 64u * NT;                        // one k16 step: hi (2 chunks) + lo
   const uint32_t b_stage_bytes = (uint32_t)(a.KB / 16) * b_step_bytes;
   uint8_t* a_base = smem_raw;
-  uint8_t* b_base = a_base + 2 * a_stage_bytes;
-  float4* pads = reinterpret_cast<float4*>(b_base + (size_t)a.NB * b_stage_bytes);   // 4 warps x [32][8] float4
-  uint64_t* bars = reinterpret_cast<uint64_t*>(pads + (a.stats ? 4 * 256 : 0));   // transpose pads only with statistics
-  // bars: a_full[2], a_empty[2], acc_full[2], acc_empty[2], b_full[NB], b_empty[NB]
+  uint8_t* b_base = a_base + (size_t)a.SA * a_stage_bytes;
+  float* tab_s = reinterpret_cast<float*>(b_base + (size_t)a.NB * b_stage_bytes);         // [2][TAB_NB][96]
+  unsigned long long* stat_s = reinterpret_cast<unsigned long long*>(tab_s + 2 * TAB_NB * 96);   // [NJ][2][NT]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stat_s + (a.stats ? a.NJ * 2 * NT : 0));
+  // bars: a_full[SA], a_empty[SA], b_full[NB], b_empty[NB]
   const uint32_t bar0 = smem_u32(bars);
   auto A_FULL = [&](int i) { return bar0 + 8u * i; };
-  auto A_EMPTY = [&](int i) { return bar0 + 8u * (2 + i); };
-  auto ACC_FULL = [&](int i) { return bar0 + 8u * (4 + i); };
-  auto ACC_EMPTY = [&](int i) { return bar0 + 8u * (6 + i); };
-  auto B_FULL = [&](int i) { return bar0 + 8u * (8 + i); };
-  auto B_EMPTY = [&](int i) { return bar0 + 8u * (8 + a.NB + i); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 30);
-  float4* tab_s = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(bars) + 256);   // [2][TAB_NB][32]
-  float* bias_s = reinterpret_cast<float*>(tab_s + 2 * TAB_NB * 32);                    // [NT]
-  unsigned long long* stat_s = reinterpret_cast<unsigned long long*>(bias_s + 256);     // [NJ][2][NT] (when a.stats)
+  auto A_EMPTY = [&](int i) { return bar0 + 8u * (a.SA + i); };
+  auto B_FULL = [&](int i) { return bar0 + 8u * (2 * a.SA + i); };
+  auto B_EMPTY = [&](int i) { return bar0 + 8u * (2 * a.SA + a.NB + i); };
+  const int groups_n = a.tiles_n / a.NPI;                 // work item t: m tile t / groups_n, n tiles of group t % groups_n
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int taps = a.ks * a.ks;
-  const int MTOT = MT * a.NACC;
 
   if (tid == 0) {
-    // one tcgen05.commit per MMA-issuing warp (= per accumulator) on the "consumed" barriers
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(A_FULL(i), NPROD); mbar_init(A_EMPTY(i), a.NACC);
-      mbar_init(ACC_FULL(i), a.NACC); mbar_init(ACC_EMPTY(i), 128);
-    }
-    for (int i = 0; i < a.NB; ++i) { mbar_init(B_FULL(i), 1); mbar_init(B_EMPTY(i), a.NACC); }
+    // consumers release a stage with one arrival per consumer warp (8)
+    for (int i = 0; i < a.SA; ++i) { mbar_init(A_FULL(i), NPROD); mbar_init(A_EMPTY(i), 8); }
+    for (int i = 0; i < a.NB; ++i) { mbar_init(B_FULL(i), 1); mbar_init(B_EMPTY(i), 8); }
     fence_barrier_init();
   }
-  if (warp == W_MMA) tmem_alloc(smem_u32(tmem_slot), (uint32_t)a.tmem_cols);
   if (a.stats)
-    for (int i = tid; i < a.NJ * 2 * a.NT; i += NTHREADS) stat_s[i] = 0ull;
-  tc_fence_before();
+    for (int i = tid; i < a.NJ * 2 * NT; i += NTHREADS) stat_s[i] = 0ull;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  long long* dbg = a.dbg ? a.dbg + (size_t)blockIdx.x * 16 : nullptr;
-  const long long t_begin = dbg ? clock64() : 0;
-#define DBG_T(var) long long var = dbg ? clock64() : 0
-#define DBG_ADD(slot, since, cond) do { if (dbg && (cond)) { long long t__ = clock64(); dbg[slot] += t__ - since; since = t__; } } while (0)
 
-  if (warp < 8) {
+  if (warp < W_LOAD) {
     // =========================== producers ===========================
-    // One thread = one slab position x all KB channels of the K-block.  Per K-block the 128 B channel runs
-    // of the thread's (<= 2, rarely 3) positions are requested up front (16 x LDG.128 in flight) BEFORE
-    // waiting for the stage to drain; the (mean, rstd*G, S) rows of the <= TAB_NB images the tile touches
-    // are staged in smem one K-block ahead; every 8-channel chunk leaves as one 16 B hi + one 16 B lo
-    // store (lanes walk positions => conflict-free).
+    // One thread = one slab position x all KB channels of the K-block at a time; the (mean, rstd*G, S) rows of the
+    // <= TAB_NB images the tile touches are staged in smem per K-block (double-buffered, one barrier per K-block).
     const int Cin = a.C0 + a.C1;
     const bool has_tab = a.tab != nullptr;
-    // slabs of <= 128 rows (1x1 convolutions on one accumulator) would leave half the producer threads idle:
-    // two threads share a row there, each taking half of the K-block's 8-channel chunks
-    const bool rsplit = a.HP <= NPROD / 2 && chunks >= 2;
-    const int hrow = rsplit ? (tid & (NPROD / 2 - 1)) : tid;
-    const int ch_lo = rsplit ? (tid / (NPROD / 2)) * (chunks / 2) : 0;
-    const int ch_hi = rsplit ? ch_lo + chunks / 2 : chunks;
     auto tile_b0_of = [&](int t) {
-      const long long q_first = (long long)(t / a.tiles_n) * MTOT - a.halo0;
+      const long long q_first = (long long)(t / groups_n) * MT - a.halo0;
       return q_first <= 0 ? 0 : (int)min((long long)(a.B - 1), q_first / a.Pimg);
     };
-    // norm-table rows of one K-block: <= TAB_NB * 32 = 256 float4, i.e. at most ONE per producer thread.
-    // Split into a register load (issued early, latency hidden behind the transform) and a smem store.
-    auto tab_load = [&](int tb0, int kb, float4& treg) {
-      if (!has_tab || tid >= a.tab_nb * a.KB) return;
-      const int bi = tid / a.KB, c = tid - bi * a.KB;
-      const int b = min(tb0 + bi, a.B - 1);
-      treg = __ldg(a.tab + (long long)b * Cin + kb * a.KB + c);
-    };
-    auto tab_store = [&](int g, const float4& treg) {           // -> buffer g & 1
-      if (!has_tab || tid >= a.tab_nb * a.KB) return;
-      const int bi = tid / a.KB, c = tid - bi * a.KB;
-      float* tb = reinterpret_cast<float*>(tab_s) + (size_t)(g & 1) * TAB_NB * 96 + bi * 96;   // [mean|rstd*G|S][32]
-      tb[c] = treg.x;
-      tb[32 + c] = treg.y * treg.z;
-      tb[64 + c] = treg.w;
-    };
-    auto emit = [&](const float4* raw, int pix, int bidx, int h, const float4* tsm, uint8_t* hi_base, uint8_t* lo_base,
-                    bool use_tab) {
-      if (pix == -2) return;
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        if (ch >= ch_lo && ch < ch_hi) {
-          uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
-          if (pix >= 0) {
-            float v[8] = {raw[2 * ch].x, raw[2 * ch].y, raw[2 * ch].z, raw[2 * ch].w,
-                          raw[2 * ch + 1].x, raw[2 * ch + 1].y, raw[2 * ch + 1].z, raw[2 * ch + 1].w};
-            if (use_tab) {
-              const float* tb = reinterpret_cast<const float*>(tsm) + bidx * 96 + ch * 8;
-              const float4 m0 = *reinterpret_cast<const float4*>(tb), m1 = *reinterpret_cast<const float4*>(tb + 4);
-              const float4 g0 = *reinterpret_cast<const float4*>(tb + 32), g1 = *reinterpret_cast<const float4*>(tb + 36);
-              const float4 s0 = *reinterpret_cast<const float4*>(tb + 64), s1 = *reinterpret_cast<const float4*>(tb + 68);
-              const float mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-              const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-              const float ss[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-#pragma unroll
-              for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - mm[e], gg[e], ss[e]);
-              if (a.act_in) silu_fast8(v);
-            }
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
-            hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-            lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-          }
-          const size_t off = ((size_t)ch * a.HP + h) * 16;
-          *reinterpret_cast<uint4*>(hi_base + off) = hv;
-          *reinterpret_cast<uint4*>(lo_base + off) = lv;
-        }
-      }
-    };
-    auto fetch = [&](float4* raw, int pix, const float* src, int cs, int cc0) {
-      if (pix >= 0) {
-        const float4* sp = reinterpret_cast<const float4*>(src + (long long)pix * cs + cc0);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (j >= ch_lo * 2 && j < ch_hi * 2) raw[j] = __ldg(sp + j);
-      }
-    };
-
     int g = 0;                                             // K-blocks produced so far (all tiles)
-    float4 treg = make_float4(0.f, 0.f, 0.f, 0.f);
-    if ((int)blockIdx.x < a.ntiles) { tab_load(tile_b0_of(blockIdx.x), 0, treg); tab_store(0, treg); }
-    const bool single = a.HP <= NPROD;                     // one slab row per thread: pipeline across K-blocks
     for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x) {
-      const long long p0 = (long long)(t / a.tiles_n) * MTOT;
+      const long long p0 = (long long)(t / groups_n) * MT;
       const int tb0 = tile_b0_of(t);
-      const bool more = t + (int)gridDim.x < a.ntiles;
-      const int tb_next = more ? tile_b0_of(t + gridDim.x) : 0;
-      int ppix[3], pb[3];
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        const int h = hrow + i * NPROD;
-        ppix[i] = -2;                                      // -2: no such slab row, -1: zero padding
-        pb[i] = 0;
-        if (h < a.HP) { int b = tb0; ppix[i] = decode_pos(a, p0 - a.halo0 + h, b); pb[i] = b - tb0; }
-      }
-      // the fused 1x1 shortcut (second segment) multiplies the centre tap only: its K-blocks stage just the
-      // MTOT rows the tile itself covers, one per thread, instead of the whole haloed slab
-      const bool centre = !single && a.nKB > a.nKB0;
-      int cpix = -2;
-      if (centre && tid < MTOT) { int b = tb0; cpix = decode_pos(a, p0 + tid, b); }
-      auto src_of = [&](int kb, const float*& src, int& cs, int& cc0) {
-        if (kb < a.nKB0) {
+      for (int kb = 0; kb < a.nKB; ++kb, ++g) {
+        const int st = g % a.SA;
+        const float* src; int cs, cc0;
+        const bool seg2 = kb >= a.nKB0;
+        if (!seg2) {
           const int c0 = kb * a.KB;
           if (c0 < a.C0) { src = a.s0; cs = a.C0; cc0 = c0; } else { src = a.s1; cs = a.C1; cc0 = c0 - a.C0; }
         } else {
           const int c0 = (kb - a.nKB0) * a.KB;
           if (c0 < a.C2) { src = a.s2; cs = a.C2; cc0 = c0; } else { src = a.s3; cs = a.C3; cc0 = c0 - a.C2; }
         }
-      };
-      // one K-block: `cur` already holds (or receives) this K-block's channels of slab row 0; when `single`,
-      // the NEXT K-block's channels are requested into `nxt` before the transform starts.
-      auto step = [&](float4* cur, float4* nxt, int kb) {
-        const int st = g & 1;
-        const float* src; int cs, cc0;
-        src_of(kb, src, cs, cc0);
-        const bool seg2 = centre && kb >= a.nKB0;
-        if (seg2) fetch(cur, cpix, src, cs, cc0);
-        else if (!single) { fetch(cur, ppix[0], src, cs, cc0); fetch(nxt, ppix[1], src, cs, cc0); }
-        else if (kb + 1 < a.nKB) { const float* s2; int cs2, cc2; src_of(kb + 1, s2, cs2, cc2); fetch(nxt, ppix[0], s2, cs2, cc2); }
-        const bool tab_now = has_tab && kb < a.nKB0;                       // this K-block is normalised
-        const bool tab_nxt = has_tab && (kb + 1 < a.nKB0 || (kb + 1 == a.nKB && more));
-        if (tab_nxt) { if (kb + 1 < a.nKB0) tab_load(tb0, kb + 1, treg); else tab_load(tb_next, 0, treg); }
-        DBG_T(tp);
-        mbar_wait(A_EMPTY(st), ((g >> 1) & 1) ^ 1);
-        DBG_ADD(1, tp, tid == 0);
-        if (tab_now) asm volatile("bar.sync 1, 256;" ::: "memory");   // this K-block's table staged by all
-        DBG_ADD(2, tp, tid == 0);
-        uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes;
-        uint8_t* lo_base = hi_base + a_half_bytes;
-        const float4* tsm = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(tab_s) + (size_t)st * TAB_NB * 96);
-        if (seg2) emit(cur, cpix, 0, a.halo0 + tid, tsm, hi_base, lo_base, false);
-        else emit(cur, ppix[0], pb[0], hrow, tsm, hi_base, lo_base, tab_now);
-        if (!single && !seg2) {
-          emit(nxt, ppix[1], pb[1], tid + NPROD, tsm, hi_base, lo_base, tab_now);
-          if (a.HP > 2 * NPROD) {                        // 128-wide images: a third slab row for some threads
-            fetch(nxt, ppix[2], src, cs, cc0);
-            emit(nxt, ppix[2], pb[2], tid + 2 * NPROD, tsm, hi_base, lo_base, tab_now);
+        const bool use_tab = has_tab && !seg2;
+        float* tsm = tab_s + (size_t)(g & 1) * TAB_NB * 96;
+        if (use_tab) {
+          for (int i = tid; i < a.tab_nb * a.KB; i += NPROD) {
+            const int bi = i / a.KB, c = i - bi * a.KB;
+            const int b = min(tb0 + bi, a.B - 1);
+            const int ch = kb * a.KB + c;
+            float m, gs, sh;
+            if (a.tab_planar) {
+              const float* tp = a.tab + (long long)b * 3 * Cin + ch;
+              m = __ldg(tp); gs = __ldg(tp + Cin); sh = __ldg(tp + 2 * Cin);
+            } else {
+              const float4 tv = __ldg(reinterpret_cast<const float4*>(a.tab) + (long long)b * Cin + ch);
+              m = tv.x; gs = tv.y * tv.z; sh = tv.w;
+            }
+            tsm[bi * 96 + c] = m; tsm[bi * 96 + 32 + c] = gs; tsm[bi * 96 + 64 + c] = sh;
           }
         }
-        DBG_ADD(3, tp, tid == 0);
-        fence_proxy_async();          // make the generic-proxy stores visible to the tensor-core proxy
-        mbar_arrive(A_FULL(st));
-        DBG_ADD(4, tp, tid == 0);
-        // table of the NEXT K-block (possibly of the next tile) into the other buffer; everyone finished
-        // reading that buffer before passing this K-block's bar.sync
-        if (tab_nxt) {
-          // a raw (second-segment) K-block has no table barrier of its own: make sure every producer is done
-          // reading the buffer about to be overwritten
-          if (!tab_now) asm volatile("bar.sync 1, 256;" ::: "memory");
-          tab_store(g + 1, treg);
+        mbar_wait(A_EMPTY(st), ((g / a.SA) & 1) ^ 1);
+        // this K-block's table is complete, and every producer finished reading the buffer written two K-blocks ago
+        named_bar_sync(1, NPROD);
+        uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes;
+        uint8_t* lo_base = hi_base + a_half_bytes;
+#pragma unroll 1
+        for (int h = tid; h < a.HP; h += NPROD) {
+          int b = tb0;
+          const int pix = decode_pos(a, p0 - a.halo0 + h, b);
+          const int bidx = b - tb0;
+          float4 raw[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (j < 2 * chunks) raw[j] = pix >= 0 ? __ldg(reinterpret_cast<const float4*>(src + (long long)pix * cs + cc0) + j)
+                                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int ch = 0; ch < 4; ++ch) {
+            if (ch < chunks) {
+              uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
+              if (pix >= 0) {
+                float v[8] = {raw[2 * ch].x, raw[2 * ch].y, raw[2 * ch].z, raw[2 * ch].w,
+                              raw[2 * ch + 1].x, raw[2 * ch + 1].y, raw[2 * ch + 1].z, raw[2 * ch + 1].w};
+                if (use_tab) {
+                  const float* tb = tsm + bidx * 96 + ch * 8;
+#pragma unroll
+                  for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tb[e], tb[32 + e], tb[64 + e]);
+                  if (a.act_in) silu_fast8(v);
+                }
+                uint32_t hw[4], lw[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
+                hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+                lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+              }
+              const size_t off = ((size_t)ch * a.HP + h) * 16;
+              *reinterpret_cast<uint4*>(hi_base + off) = hv;
+              *reinterpret_cast<uint4*>(lo_base + off) = lv;
+            }
+          }
         }
-        ++g;
-      };
-      float4 rawA[8], rawB[8];
-      if (single) { const float* s0; int cs0, cc0; src_of(0, s0, cs0, cc0); fetch(rawA, ppix[0], s0, cs0, cc0); }
-      for (int kb = 0; kb < a.nKB; kb += 2) {
-        step(rawA, rawB, kb);
-        if (kb + 1 < a.nKB) step(rawB, rawA, kb + 1);
+        fence_proxy_async();          // make the generic-proxy stores visible to the tensor-core (async) proxy
+        mbar_arrive(A_FULL(st));
       }
     }
   } else if (warp == W_LOAD) {
@@ -329,8 +224,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const UmmaArgs a) {
       const uint32_t b0 = smem_u32(b_base);
       const int per_tile = a.nKB0 * taps + (a.nKB - a.nKB0);          // second segment: one (centre) tap per K-block
       int st = 0, ph = 1;
-      for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x) {
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wpk) + (size_t)(t % a.tiles_n) * per_tile * b_stage_bytes;
+      for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x)
+       for (int j = 0; j < a.NPI; ++j) {
+        const int nt = (t % groups_n) * a.NPI + j;
+        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wpk) + (size_t)nt * per_tile * b_stage_bytes;
         for (int i = 0; i < per_tile; ++i) {
           mbar_wait(B_EMPTY(st), ph);
           mbar_arrive_expect_tx(B_FULL(st), b_stage_bytes);
@@ -340,300 +237,148 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const UmmaArgs a) {
       }
     }
     __syncwarp();
-  } else if (warp == W_MMA || warp == W_MMA2) {
-    // =========================== MMA issuers ===========================
-    // warp W_MMA feeds accumulator 0, warp W_MMA2 accumulator 1 (idle for one-accumulator tiles); both wait for the
-    // same slab / weight stages and each commits "consumed" for its own MMAs
-    const int my_acc = (warp == W_MMA) ? 0 : 1;
-    if (my_acc < a.NACC && elect_one()) {
-      const uint32_t idesc = make_idesc_f16(MT, a.NT);
-      const uint32_t a_lbo16 = (uint32_t)a.HP, b_lbo16 = (uint32_t)a.NT;      // LBO in 16-byte units
-      const uint64_t a_proto = make_desc(0, a_lbo16 * 16, 128), b_proto = make_desc(0, b_lbo16 * 16, 128);
-      const int ksteps = a.KB / 16;
-      const uint32_t a_half16 = a_half_bytes >> 4, b_step16 = b_step_bytes >> 4, b_lo16 = 2u * a.NT;
-      const uint32_t a0_16 = smem_u32(a_base) >> 4, b0_16 = smem_u32(b_base) >> 4;
-      const uint32_t a_stage16 = a_stage_bytes >> 4, b_stage16 = b_stage_bytes >> 4;
-      int bst = 0, bph = 0, g = 0, it = 0;
-      for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x, ++it) {
-        const int set = it % a.nsets;
-        DBG_T(tm);
-        mbar_wait(ACC_EMPTY(set), ((it / a.nsets) & 1) ^ 1);      // epilogue drained this accumulator set
-        DBG_ADD(5, tm, my_acc == 0);
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + (uint32_t)(set * a.NACC * a.NT);
-        uint32_t accum = 0;                    // 0 only for the very first MMA of each accumulator
-        for (int kb = 0; kb < a.nKB; ++kb, ++g) {
-          const int st = g & 1;
-          DBG_ADD(8, tm, my_acc == 0);
-          mbar_wait(A_FULL(st), (g >> 1) & 1);
-          DBG_ADD(6, tm, my_acc == 0);
-          tc_fence_after();
-          const uint32_t a_hi16 = a0_16 + (uint32_t)st * a_stage16 + (uint32_t)a.halo0;
-          const int ntap = (kb < a.nKB0) ? taps : 1;
-          for (int tap = 0; tap < ntap; ++tap) {
-            DBG_ADD(8, tm, my_acc == 0);
-            mbar_wait(B_FULL(bst), bph);
-            DBG_ADD(7, tm, my_acc == 0);
-            tc_fence_after();
-            const int shift = (a.ks == 3 && kb < a.nKB0) ? ((tap / 3 - 1) * a.Wp + (tap % 3 - 1)) : 0;
-            const uint32_t a_tap16 = a_hi16 + (uint32_t)shift;
-            const uint32_t b_tap16 = b0_16 + (uint32_t)bst * b_stage16;
-            for (int s = 0; s < ksteps; ++s) {
-              const uint64_t dbh = desc_add(b_proto, b_tap16 + (uint32_t)s * b_step16);
-              const uint64_t dbl = desc_add(dbh, b_lo16);
-              const uint32_t a_s16 = a_tap16 + (uint32_t)(2 * s) * a_lbo16;
-              {
-                const uint64_t dah = desc_add(a_proto, a_s16 + (uint32_t)(my_acc * MT));
-                const uint64_t dal = desc_add(dah, a_half16);
-                const uint32_t d = d0 + (uint32_t)(my_acc * a.NT);
-                umma_f16(d, dah, dbh, idesc, accum);
-                if (a.split & 1) umma_f16(d, dal, dbh, idesc, 1u);
-                if (a.split & 2) umma_f16(d, dah, dbl, idesc, 1u);
-              }
-              accum = 1u;
-            }
-            umma_commit(B_EMPTY(bst));        // weights of this stage consumed
-            if (++bst == a.NB) { bst = 0; bph ^= 1; }
-          }
-          umma_commit(A_EMPTY(st));           // slab of this K-block consumed
-        }
-        umma_commit(ACC_FULL(set));
-        DBG_ADD(8, tm, my_acc == 0);
-      }
-    }
-    __syncwarp();
   } else {
-    // =========================== epilogue ===========================
-    // Each of the 4 warps drains its 32 TMEM lanes (rows) in column blocks of 32 (or a 16-wide tail): the
-    // block is transposed through an XOR-swizzled 4 KB shared-memory pad so that every global load / store
-    // instruction covers whole 128-byte lines of `dst` / `res` (8 lanes per row).
-    const int lq = warp & 3;
-    const int et = tid - W_EPI * 32;                           // 0..127 within the epilogue group
-    float4* pad = pads + (size_t)(warp - W_EPI) * 256;        // [32 rows][8 float4]
-    const int nblk = (a.NT + 31) / 32;
-    const float* __restrict__ resp = a.res;
-    float* __restrict__ dstp = a.dst;
-    int it = 0;
-    for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x, ++it) {
-      const int set = it % a.nsets;
-      const long long p0 = (long long)(t / a.tiles_n) * MTOT;
-      const int n0 = (t % a.tiles_n) * a.NT;
-      // bias of this n-tile -> smem (read back as broadcast float4s); guarded by the group's named barrier
-      asm volatile("bar.sync 2, 128;" ::: "memory");           // previous tile's readers are done
-      for (int i = et; i < a.NT; i += 128) bias_s[i] = a.bias ? __ldg(a.bias + n0 + i) : 0.f;
-      asm volatile("bar.sync 2, 128;" ::: "memory");
-      if (resp && !a.stats) {
-        // the residual rows of this tile are pulled into L2 while its MMAs are still running (the epilogue warps
-        // would only be waiting): the drain below then pays an L2 hit per block instead of a DRAM round trip
-        for (int acc = 0; acc < a.NACC; ++acc) {
-          int bb = 0;
-          const int px = decode_pos(a, p0 + (long long)acc * MT + lq * 32 + lane, bb);
-          if (px >= 0) {
-            const float* rp = resp + (long long)px * a.Cout + n0;
-            for (int c = 0; c < a.NT; c += 32) prefetch_l2(rp + c);
+    // =========================== consumers (MMA + epilogue) ===========================
+    const int wg = (warp - W_CONS) >> 2;                   // rows [64 wg, 64 wg + 64) of the tile
+    const int wq = (warp - W_CONS) & 3;                             // warp within the warpgroup: rows 16 wq .. 16 wq + 15
+    const int ksteps = a.KB / 16;
+    const uint32_t a_lbo = (uint32_t)a.HP * 16;
+    const uint64_t a_proto = make_desc(0, a_lbo, 128), b_proto = make_desc(0, NT * 16, 128);
+    const uint32_t a_half16 = a_half_bytes >> 4, b_lo16 = 2u * NT;
+    const uint32_t a0_16 = smem_u32(a_base) >> 4, b0_16 = smem_u32(b_base) >> 4;
+    const uint32_t a_stage16 = a_stage_bytes >> 4, b_stage16 = b_stage_bytes >> 4;
+    const uint32_t a_lbo16 = a_lbo >> 4;
+    int bst = 0, bph = 0, g0 = 0;                          // g0: first K-block (all items) of the current item
+    for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x, g0 += a.nKB)
+     for (int j = 0; j < a.NPI; ++j) {
+      const long long p0 = (long long)(t / groups_n) * MT;
+      const int n0 = ((t % groups_n) * a.NPI + j) * NT;
+      const bool last_n = j == a.NPI - 1;                  // the slab stages are released after the item's last n tile
+      float acc[NT / 2];
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+      // the stage whose wgmmas were committed last and not yet released (one group stays in flight)
+      int pend_b = -1, pend_a = -1;
+      for (int kb = 0; kb < a.nKB; ++kb) {
+        const int g = g0 + kb;
+        const int st = g % a.SA;
+        mbar_wait(A_FULL(st), (g / a.SA) & 1);
+        const uint32_t a_hi16 = a0_16 + (uint32_t)st * a_stage16 + (uint32_t)(a.halo0 + 64 * wg);
+        const int ntap = (kb < a.nKB0) ? taps : 1;
+        for (int tap = 0; tap < ntap; ++tap) {
+          mbar_wait(B_FULL(bst), bph);
+          const int shift = (a.ks == 3 && kb < a.nKB0) ? ((tap / 3 - 1) * a.Wp + (tap % 3 - 1)) : 0;
+          const uint32_t a_tap16 = a_hi16 + (uint32_t)shift;
+          const uint32_t b_tap16 = b0_16 + (uint32_t)bst * b_stage16;
+          wgmma_fence();
+#pragma unroll 1
+          for (int s = 0; s < ksteps; ++s) {
+            const uint64_t dbh = desc_add(b_proto, b_tap16 + (uint32_t)s * (b_step_bytes >> 4));
+            const uint64_t dbl = desc_add(dbh, b_lo16);
+            const uint64_t dah = desc_add(a_proto, a_tap16 + (uint32_t)(2 * s) * a_lbo16);
+            const uint64_t dal = desc_add(dah, a_half16);
+            wgmma_ss<NT>(acc, dah, dbh, 1);
+            if (a.split & 1) wgmma_ss<NT>(acc, dal, dbh, 1);
+            if (a.split & 2) wgmma_ss<NT>(acc, dah, dbl, 1);
           }
+          wgmma_commit();
+          wgmma_wait<1>();                                 // the previous group is complete: release its stages
+          if (pend_b >= 0 && lane == 0) mbar_arrive(B_EMPTY(pend_b));
+          if (pend_a >= 0 && lane == 0) mbar_arrive(A_EMPTY(pend_a));
+          pend_b = bst;
+          pend_a = (tap == ntap - 1 && last_n) ? st : -1;
+          if (++bst == a.NB) { bst = 0; bph ^= 1; }
         }
       }
-      DBG_T(te);
-      mbar_wait(ACC_FULL(set), (it / a.nsets) & 1);
-      DBG_ADD(9, te, tid == W_EPI * 32);
-      tc_fence_after();
-      const uint32_t trow0 = tmem_base + ((uint32_t)(lq * 32) << 16) + (uint32_t)(set * a.NACC * a.NT);
-      for (int acc = 0; acc < a.NACC; ++acc) {
-        int myb = 0;
-        const int mypix = decode_pos(a, p0 + (long long)acc * MT + lq * 32 + lane, myb);
-        if (!a.stats) {
-          // Row-per-lane drain (round 2, as in conv1x1_umma.cu): the lane writes the columns of its own position as
-          // 256-bit stores -- whole 32-byte sectors, no shared-memory transpose, a third of the instructions; the
-          // residual of a block is requested before the TMEM load is waited for.
-          const bool ok = mypix >= 0;
-          float* orow = dstp + (long long)mypix * a.Cout + n0;
-          const float* rrow = (resp && ok) ? resp + (long long)mypix * a.Cout + n0 : nullptr;
-          for (int blk = 0; blk < nblk; ++blk) {
-            const int cb = blk * 32;
-            const int w = min(32, a.NT - cb);               // 32 or 16 columns
-            float rr[32];
-            if (rrow) {
+      wgmma_wait<0>();
 #pragma unroll
-              for (int c8 = 0; c8 < 4; ++c8)
-                if (c8 * 8 < w) ldg256(rrow + cb + c8 * 8, rr + c8 * 8);
-            }
-            uint32_t r[32];
-            tmem_ld16(trow0 + (uint32_t)(acc * a.NT + cb), r);
-            if (w == 32) tmem_ld16(trow0 + (uint32_t)(acc * a.NT + cb + 16), r + 16);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-              if (c8 * 8 < w) {
-                const float4 b0 = *reinterpret_cast<const float4*>(bias_s + cb + c8 * 8);
-                const float4 b1 = *reinterpret_cast<const float4*>(bias_s + cb + c8 * 8 + 4);
-                const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                float v[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                  v[e] = __uint_as_float(r[c8 * 8 + e]) * a.wscale + bb[e];    // wscale is a power of two: exact product
-                  if (rrow) v[e] += rr[c8 * 8 + e];
-                  v[e] *= a.oscale;
-                  if (a.act_out) v[e] = silu_f(v[e]);
-                }
-                if (ok) stg256(orow + cb + c8 * 8, v);
-              }
-            }
-          }
-          continue;
-        }
-        // statistics: image slot of this row inside its 128-position tile, and the slots present in this warp
-        const long long q_tile = p0 + (long long)acc * MT;
-        const int tile_b0 = (int)min((long long)(a.B - 1), q_tile / a.Pimg);
-        const int myj = mypix >= 0 ? myb - tile_b0 : -1;
-        unsigned jmask = 0;
-        if (a.stats) {
-#pragma unroll 1
-          for (int jj = 0; jj < 4; ++jj)
-            if (__ballot_sync(0xffffffffu, myj == jj)) jmask |= 1u << jj;
-        }
-        // per-(slot, channel) sums of this warp's rows of one column block -> the CTA's shared accumulators
-        auto stat_block = [&](int cb, int lpr, int qc, int rsub, int rpi) {
-#pragma unroll 1
-          for (int jj = 0; jj < 4; ++jj) {
-            if (!(jmask & (1u << jj))) continue;
-            long long s1[4] = {0, 0, 0, 0};
-            unsigned long long s2[4] = {0, 0, 0, 0};
-#pragma unroll 2
-            for (int row = rsub; row < 32; row += rpi) {
-              if (__shfl_sync(0xffffffffu, myj, row) == jj) {
-                const float4 t = pad[row * 8 + (qc ^ (row & 7))];
-                const float f[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const int xi = __float2int_rn(f[e] * STAT_SCALE);       // saturates at +-2^31
-                  s1[e] += xi;
-                  s2[e] += (unsigned long long)((long long)xi * (long long)xi);
-                }
-              }
-            }
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              for (int o = lpr; o <= 16; o <<= 1) {
-                s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], o);
-                s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], o);
-              }
-            }
-            if (lane < lpr) {
-              unsigned long long* sp = stat_s + (size_t)jj * 2 * a.NT + cb + qc * 4;
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                atomicAdd(sp + e, (unsigned long long)s1[e]);
-                atomicAdd(sp + a.NT + e, s2[e]);
-              }
-            }
-          }
-        };
-        // row slots of this lane in the transposed (coalesced) phase, for 32-wide blocks: 8 lanes per row
-        int px8[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) px8[k] = __shfl_sync(0xffffffffu, mypix, k * 4 + (lane >> 3));
-        const int q8 = lane & 7;
-        float4 rnext[8];
-        auto res_fetch = [&](int blk) {                       // residual of a full 32-wide block -> registers
-          if (!resp) return;
-          const int cb = blk * 32;
-#pragma unroll
-          for (int k = 0; k < 8; ++k)
-            if (px8[k] >= 0) rnext[k] = __ldg(reinterpret_cast<const float4*>(resp + (long long)px8[k] * a.Cout + n0 + cb + q8 * 4));
-        };
-        if (a.NT >= 32) res_fetch(0);
-        for (int blk = 0; blk < nblk; ++blk) {
-          const int cb = blk * 32;
-          const int w = min(32, a.NT - cb);                 // 32 or 16 columns
-          uint32_t r[32];
-          tmem_ld16(trow0 + (uint32_t)(acc * a.NT + cb), r);
-          if (w == 32) tmem_ld16(trow0 + (uint32_t)(acc * a.NT + cb + 16), r + 16);
-          tmem_ld_wait();
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            if (q * 4 < w)
-              pad[lane * 8 + (q ^ (lane & 7))] =
-                  make_float4(__uint_as_float(r[4 * q]) * a.wscale, __uint_as_float(r[4 * q + 1]) * a.wscale,
-                              __uint_as_float(r[4 * q + 2]) * a.wscale, __uint_as_float(r[4 * q + 3]) * a.wscale);
-          __syncwarp();
-          if (w == 32) {
-            float4 rcur[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) rcur[k] = rnext[k];
-            if ((blk + 1) * 32 + 32 <= a.NT) res_fetch(blk + 1);      // next full block's residual in flight
-            const float4 bv = *reinterpret_cast<const float4*>(bias_s + cb + q8 * 4);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const int row = k * 4 + (lane >> 3);
-              if (px8[k] >= 0) {
-                float4 v = pad[row * 8 + (q8 ^ (row & 7))];
-                v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-                if (resp) { v.x += rcur[k].x; v.y += rcur[k].y; v.z += rcur[k].z; v.w += rcur[k].w; }
-                v.x *= a.oscale; v.y *= a.oscale; v.z *= a.oscale; v.w *= a.oscale;
-                if (a.act_out) { v.x = silu_f(v.x); v.y = silu_f(v.y); v.z = silu_f(v.z); v.w = silu_f(v.w); }
-                *reinterpret_cast<float4*>(dstp + (long long)px8[k] * a.Cout + n0 + cb + q8 * 4) = v;
-                if (a.stats) pad[row * 8 + (q8 ^ (row & 7))] = v;        // re-read by stat_block (same thread)
-              }
-            }
-            if (a.stats) stat_block(cb, 8, q8, lane >> 3, 4);
-          } else {                                          // 16-wide tail: 4 lanes per row, 8 rows per instruction
-            const int q = lane & 3, rsub = lane >> 2;
-            const float4 bv = *reinterpret_cast<const float4*>(bias_s + cb + q * 4);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int row = k * 8 + rsub;
-              const int px = __shfl_sync(0xffffffffu, mypix, row);
-              if (px >= 0) {
-                float4 v = pad[row * 8 + (q ^ (row & 7))];
-                v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-                const long long off = (long long)px * a.Cout + n0 + cb + q * 4;
-                if (resp) {
-                  const float4 rv = __ldg(reinterpret_cast<const float4*>(resp + off));
-                  v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
-                }
-                v.x *= a.oscale; v.y *= a.oscale; v.z *= a.oscale; v.w *= a.oscale;
-                if (a.act_out) { v.x = silu_f(v.x); v.y = silu_f(v.y); v.z = silu_f(v.z); v.w = silu_f(v.w); }
-                *reinterpret_cast<float4*>(dstp + off) = v;
-                if (a.stats) pad[row * 8 + (q ^ (row & 7))] = v;
-              }
-            }
-            if (a.stats) stat_block(cb, 4, q, rsub, 8);
-          }
-          __syncwarp();
-        }
-        if (a.stats) {
-          // the four warps' sums of this 128-position tile -> global [tile128][NJ][2][Cout]; re-zero for the next tile
-          asm volatile("bar.sync 2, 128;" ::: "memory");
-          const long long tile128 = q_tile / MT;
-          unsigned long long* gp = a.stats + (size_t)tile128 * a.NJ * 2 * a.Cout;
-          for (int i = et; i < a.NJ * 2 * a.NT; i += 128) {
-            const int jp = i / a.NT, n = i - jp * a.NT;
-            gp[(size_t)jp * a.Cout + n0 + n] = stat_s[i];
-            stat_s[i] = 0ull;
-          }
-          asm volatile("bar.sync 2, 128;" ::: "memory");
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(ACC_EMPTY(set));            // 128 arrivals: this accumulator set may be overwritten
-      DBG_ADD(10, te, tid == W_EPI * 32);
-    }
-  }
+      for (int i = 0; i < NT / 2; ++i) reg_fence(acc[i]);
+      if (lane == 0) { mbar_arrive(B_EMPTY(pend_b)); if (pend_a >= 0) mbar_arrive(A_EMPTY(pend_a)); }
 
-  __syncthreads();
-  if (dbg && tid == 0) dbg[0] = clock64() - t_begin;
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
+      // ---- epilogue: thread owns rows r and r + 8, two adjacent columns of every 8-column block ----
+      const int r0 = 64 * wg + 16 * wq + (lane >> 2);
+      const int cq = 2 * (lane & 3);
+      int pix[2], slot[2];
+      const int tile_b0 = (int)min((long long)(a.B - 1), p0 / a.Pimg);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        int b = 0;
+        pix[i] = decode_pos(a, p0 + r0 + 8 * i, b);
+        slot[i] = pix[i] >= 0 ? b - tile_b0 : -1;
+      }
+      unsigned jmask = 0;
+      if (a.stats) {
+#pragma unroll 1
+        for (int jj = 0; jj < a.NJ; ++jj)
+          if (__ballot_sync(0xffffffffu, slot[0] == jj || slot[1] == jj)) jmask |= 1u << jj;
+      }
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        const int n = n0 + 8 * j + cq;
+        const float2 bv = a.bias ? __ldg(reinterpret_cast<const float2*>(a.bias + n)) : make_float2(0.f, 0.f);
+        float v[2][2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float2 rv = make_float2(0.f, 0.f);
+          if (a.res && pix[i] >= 0) rv = __ldg(reinterpret_cast<const float2*>(a.res + (long long)pix[i] * a.Cout + n));
+          float x0 = (acc[4 * j + 2 * i] * a.wscale + bv.x + rv.x) * a.oscale;     // wscale: power of two, exact
+          float x1 = (acc[4 * j + 2 * i + 1] * a.wscale + bv.y + rv.y) * a.oscale;
+          if (a.act_out) { x0 = silu_f(x0); x1 = silu_f(x1); }
+          v[i][0] = x0; v[i][1] = x1;
+          if (pix[i] >= 0) *reinterpret_cast<float2*>(a.dst + (long long)pix[i] * a.Cout + n) = make_float2(x0, x1);
+        }
+        if (a.stats) {
+#pragma unroll 1
+          for (int jj = 0; jj < a.NJ; ++jj) {
+            if (!(jmask & (1u << jj))) continue;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              long long s1 = 0;
+              unsigned long long s2 = 0;
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                if (slot[i] == jj) {
+                  const int xi = __float2int_rn(v[i][e] * STAT_SCALE);          // saturates at +-2^31
+                  s1 += xi;
+                  s2 += (unsigned long long)((long long)xi * (long long)xi);
+                }
+              }
+#pragma unroll
+              for (int o = 4; o <= 16; o <<= 1) {
+                s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+                s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+              }
+              if (lane < 4) {
+                unsigned long long* sp = stat_s + (size_t)jj * 2 * NT + 8 * j + cq + e;
+                atomicAdd(sp, (unsigned long long)s1);
+                atomicAdd(sp + NT, s2);
+              }
+            }
+          }
+        }
+      }
+      if (a.stats) {
+        // both warpgroups' sums of this 128-position tile -> global [tile128][NJ][2][Cout]; re-zero for the next tile
+        named_bar_sync(2, 256);
+        const int et = tid - W_CONS * 32;
+        unsigned long long* gp = a.stats + (size_t)(p0 / MT) * a.NJ * 2 * a.Cout;
+        for (int i = et; i < a.NJ * 2 * NT; i += 256) {
+          const int jp = i / NT, n = i - jp * NT;
+          gp[(size_t)jp * a.Cout + n0 + n] = stat_s[i];
+          stat_s[i] = 0ull;
+        }
+        named_bar_sync(2, 256);
+      }
+    }
   }
 }
 
 // ---- weight packing ---------------------------------------------------------------------------------
 // in : w_taps fp32 [taps][Cin][Cout]
-// out: fp16, for nt, kb, tap, s(k16):  hi[2 chunks][NT][8]  then  lo[2 chunks][NT][8]
+// out: fp16 stages of (KB/16) k16 steps, each  hi[2 chunks][NT][8]  then  lo[2 chunks][NT][8]; stage of
+//      (n tile nt, K-block kb, tap) = nt * per_unit + stage_off + kb * taps + tap
 __global__ void k_pack_weights(const float* __restrict__ w, __half* __restrict__ out, int taps, int Cin, int Cout,
-                               int NT, int KB, float scale) {
+                               int NT, int KB, float scale, int stage_off, int per_unit) {
   const int ksteps = KB / 16, nKB = Cin / KB, nNT = Cout / NT;
   const long long total = (long long)nNT * nKB * taps * ksteps * 2 * NT * 8;  // (chunk j, n, e) per step
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -650,7 +395,7 @@ __global__ void k_pack_weights(const float* __restrict__ w, __half* __restrict__
     float v = w[((long long)tap * Cin + c) * Cout + nt * NT + n] * scale;
     __half h = __float2half_rn(v);
     __half l = __float2half_rn(v - __half2float(h));
-    long long step = (((long long)nt * nKB + kb) * taps + tap) * ksteps + s;
+    long long step = ((long long)nt * per_unit + stage_off + (long long)kb * taps + tap) * ksteps + s;
     long long base = step * (4LL * NT * 8);      // halfs per step: hi 2*NT*8 + lo 2*NT*8
     long long o = (long long)(j * NT + n) * 8 + e;
     out[base + o] = h;
@@ -664,88 +409,154 @@ int pick_kb(int C0, int C1) {
   return 0;
 }
 
-}  // namespace
+// K-block of a conv with a (C0|C1) main source and an optional (C2|C3) shortcut segment; 0 = not runnable
+int conv_kb(int C0, int C1, int C2, int C3) {
+  int kb = pick_kb(C0, C1);
+  if (C2 + C3 > 0 && pick_kb(C2, C3) < kb) kb = pick_kb(C2, C3);
+  return kb;
+}
 
-int launch_conv_umma(const McvdOp& op, cudaStream_t s) {
-  MCVD_CHECK(op.src0 && op.w && op.dst && (op.C1 == 0 || op.src1), "CONV_UMMA: null pointer");
-  MCVD_CHECK(op.i0 == 1 || op.i0 == 3, "CONV_UMMA: kernel size %d unsupported", op.i0);
-  {
-    int rc = 0;                                  // plain 1x1 convolutions: input-stationary kernel (conv1x1_umma.cu)
-    if (try_launch_conv1x1(op, s, rc)) return rc;
-  }
-  UmmaArgs a;
+struct Plan {
+  int HP, NB, NJ;
+  size_t smem;
+};
+
+constexpr size_t SMEM_LIMIT = 227 * 1024;
+
+// shared-memory plan of one conv with SA slab stages; false when it does not fit
+bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, Plan& p) {
+  const int Wp = ks == 3 ? W + 1 : W;
+  const int Pimg = ks == 3 ? (H + 1) * (W + 1) : H * W;
+  const int halo0 = ks == 3 ? Wp + 1 : 0;
+  p.HP = (MT + 2 * halo0 + 7) & ~7;
+  p.NJ = (MT - 1) / Pimg + 2;
+  if (p.HP > HP_MAX) return false;
+  const size_t a_stage = (size_t)2 * (KB / 8) * p.HP * 16;
+  const size_t b_stage = (size_t)(KB / 16) * 64 * NT;
+  const size_t stat_bytes = stats ? (size_t)p.NJ * 2 * NT * 8 : 0;
+  const size_t fixed = SA * a_stage + (size_t)2 * TAB_NB * 96 * 4 + stat_bytes + 8 * (2 * SA + 20);   // ... + barriers
+  if (fixed + 2 * b_stage > SMEM_LIMIT) return false;
+  p.NB = (int)((SMEM_LIMIT - fixed) / b_stage);
+  if (p.NB > 10) p.NB = 10;
+  p.smem = fixed + (size_t)p.NB * b_stage;
+  return true;
+}
+
+template <int NT>
+int launch_nt(const ConvArgs& a, size_t smem, int grid, cudaStream_t s) {
+  cudaError_t e = cudaFuncSetAttribute(k_conv_umma<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  MCVD_CHECK(e == cudaSuccess, "CONV_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+  k_conv_umma<NT><<<grid, NTHREADS, smem, s>>>(a);
+  MCVD_CUDA_LAUNCH_CHECK("conv_umma");
+  return 0;
+}
+
+// common launcher: planar = the CONV_UMMA2 variant (planar norm table, K-block fixed by the caller when i2 != 0,
+// statistics tiles padded to pairs)
+int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
+  const char* name = planar ? "CONV_UMMA2" : "CONV_UMMA";
+  MCVD_CHECK(op.src0 && op.w && op.dst && (op.C1 == 0 || op.src1), "%s: null pointer", name);
+  MCVD_CHECK(op.i0 == 1 || op.i0 == 3, "%s: kernel size %d unsupported", name, op.i0);
+  ConvArgs a;
   a.s0 = (const float*)op.src0; a.s1 = (const float*)op.src1; a.wpk = (const __half*)op.w;
   a.s2 = (const float*)op.src2; a.s3 = (const float*)op.src3; a.C2 = op.src2 ? op.C2 : 0; a.C3 = op.src3 ? op.C3 : 0;
-  a.bias = (const float*)op.bias; a.res = (const float*)op.aux0; a.tab = (const float4*)op.aux1;
+  a.bias = (const float*)op.bias; a.res = (const float*)op.aux0; a.tab = (const float*)op.aux1;
+  a.tab_planar = planar ? 1 : 0;
   a.dst = (float*)op.dst;
   a.stats = (unsigned long long*)op.dst2;
-  a.dbg = (long long*)op.aux2;
   a.B = op.B; a.H = op.H; a.W = op.W; a.C0 = op.C0; a.C1 = op.C1; a.Cout = op.Cout; a.ks = op.i0;
-  a.NT = op.i1;
-  a.KB = pick_kb(op.C0, op.C1);
-  if (a.C2 + a.C3 > 0 && pick_kb(a.C2, a.C3) < a.KB) a.KB = pick_kb(a.C2, a.C3);
-  MCVD_CHECK(a.KB != 0, "CONV_UMMA: input channels (%d,%d | %d,%d) must be multiples of 16", op.C0, op.C1, a.C2, a.C3);
-  MCVD_CHECK(a.NT >= 16 && a.NT <= 256 && a.NT % 16 == 0 && op.Cout % a.NT == 0,
-             "CONV_UMMA: n tile %d invalid for Cout %d", a.NT, op.Cout);
+  const int NT = op.i1;
+  a.KB = conv_kb(op.C0, op.C1, a.C2, a.C3);
+  MCVD_CHECK(a.KB != 0, "%s: input channels (%d,%d | %d,%d) must be multiples of 16", name, op.C0, op.C1, a.C2, a.C3);
+  MCVD_CHECK(!planar || op.i2 == 0 || op.i2 == a.KB, "CONV_UMMA2: weights packed for K-block %d, the conv uses %d",
+             op.i2, a.KB);
+  MCVD_CHECK(NT >= 16 && NT <= 256 && NT % 16 == 0 && op.Cout % NT == 0, "%s: n tile %d invalid for Cout %d", name, NT,
+             op.Cout);
   if (a.ks == 3) { a.Wp = op.W + 1; a.Pimg = (op.H + 1) * (op.W + 1); }
   else { a.Wp = op.W; a.Pimg = op.H * op.W; }
   a.Qtot = (long long)op.B * a.Pimg;
-  MCVD_CHECK((long long)op.B * op.H * op.W < (1LL << 31) && a.Qtot < (1LL << 31), "CONV_UMMA: too many pixels");
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  a.tiles_n = op.Cout / a.NT;
-  // accumulators per tile: i2 = 1|2 explicit, 0 = auto (2 when the double-buffered pair fits TMEM and the
-  // grid still fills the machine)
-  a.NACC = op.i2;
-  if (a.NACC == 0) {
-    // two accumulators (256-row tiles) halve the weight traffic per MAC and keep all 8 producer warps busy on
-    // 1x1 convs; fall back to 128-row tiles when that would leave SMs idle
-    a.NACC = (2 * 2 * a.NT <= 512) ? 2 : 1;      // only when the double-buffered pair still fits TMEM (measured)
-    if (a.NACC == 2 && ((a.Qtot + 2 * MT - 1) / (2 * MT)) * a.tiles_n < (long long)sms * 9 / 10) a.NACC = 1;
-  }
-  MCVD_CHECK(a.NACC == 1 || a.NACC == 2, "CONV_UMMA: accumulators %d", a.NACC);
-  a.nsets = (2 * a.NACC * a.NT <= 512) ? 2 : 1;
-  const int MTOT = MT * a.NACC;
+  MCVD_CHECK((long long)op.B * op.H * op.W < (1LL << 31) && a.Qtot < (1LL << 31), "%s: too many pixels", name);
+  MCVD_CHECK(!a.stats || a.Pimg >= 64, "%s: epilogue statistics need images of >= 64 positions", name);
   a.halo0 = (a.ks == 3) ? a.Wp + 1 : 0;
-  a.HP = (MTOT + 2 * a.halo0 + 7) & ~7;
-  MCVD_CHECK(a.HP <= 3 * NPROD, "CONV_UMMA: image width %d too large for the slab", op.W);
   a.nKB0 = (op.C0 + op.C1) / a.KB;
   a.nKB = a.nKB0 + (a.C2 + a.C3) / a.KB;
+  a.tiles_n = op.Cout / NT;
+  long long tiles_m = (a.Qtot + MT - 1) / MT;
+  if (planar) tiles_m = (tiles_m + 1) & ~1LL;          // the statistics array is sized in tile pairs: write all of it
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  // Work organisation (CONV_UMMA i2): 1 = streaming, one (m tile, n tile) per work item through two slab stages;
+  // 2 = input-stationary, one m tile per work item with its whole input resident (one slab stage per K-block) while
+  // the weights of every n tile stream past it, so the input is read and transformed once instead of once per n
+  // tile (1x1 convs without a second segment, <= MAX_RESIDENT K-blocks; otherwise streaming).  0 = input-stationary
+  // where it applies and there are at least half as many m tiles as SMs, else streaming.  Measured per 1x1 conv of
+  // cfg2 (B = 64) on an H100 80GB HBM3 (700 W), streaming -> input-stationary: 32x32 192->576 359 -> 260 us,
+  // 16x16 288->864 231 -> 130 us (128 m tiles), 8x8 288->288 37 -> 49 us (32 m tiles: too few work items).
+  // tools/time_conv1x1.py repeats the measurement.
+  const int mode = planar ? 0 : op.i2;
+  MCVD_CHECK(mode >= 0 && mode <= 2, "%s: work organisation %d", name, mode);
+  Plan p;
+  const bool can_stay = a.ks == 1 && a.nKB == a.nKB0 && a.tiles_n > 1 && a.nKB <= MAX_RESIDENT &&
+                        make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, p);
+  const bool stay = can_stay && (mode == 2 || (mode == 0 && 2 * tiles_m >= sms));
+  a.SA = stay ? a.nKB : 2;
+  a.NPI = stay ? a.tiles_n : 1;
+  MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, p),
+             "%s: tile does not fit shared memory (W=%d)", name, op.W);
+  a.HP = p.HP; a.NB = p.NB; a.NJ = p.NJ;
   a.act_in = (op.flags & MCVD_F_ACT_IN) ? 1 : 0;
   a.act_out = (op.flags & MCVD_F_ACT_OUT) ? 1 : 0;
   a.wscale = op.f1; a.oscale = op.f0;
   a.split = (op.i3 >= 1 && op.i3 <= 3) ? op.i3 : (op.i3 == 4 ? 0 : 3);
-  int cols = a.nsets * a.NACC * a.NT, p2 = 32;
-  while (p2 < cols) p2 <<= 1;
-  MCVD_CHECK(p2 <= 512, "CONV_UMMA: %d TMEM columns", cols);
-  a.tmem_cols = p2;
   {
-    int nb = a.HP / a.Pimg + 2;
-    MCVD_CHECK(nb <= TAB_NB || !a.tab, "CONV_UMMA: %dx%d images are too small for the fused-norm path", op.H, op.W);
+    const int nb = a.HP / a.Pimg + 2;
+    MCVD_CHECK(nb <= TAB_NB || !a.tab, "%s: %dx%d images are too small for the fused-norm path", name, op.H, op.W);
     a.tab_nb = (nb <= TAB_NB) ? nb : 0;
   }
-  a.NJ = (MT - 1) / a.Pimg + 2;
-  MCVD_CHECK(!a.stats || a.Pimg >= 64, "CONV_UMMA: epilogue statistics need images of >= 64 positions");
-  const size_t a_stage = (size_t)2 * (a.KB / 8) * a.HP * 16;
-  const size_t b_stage = (size_t)(a.KB / 16) * 64 * a.NT;
-  const size_t stat_bytes = a.stats ? (size_t)a.NJ * 2 * a.NT * 8 : 0;
-  const size_t fixed = 2 * a_stage + (a.stats ? 4 * 4096 : 0) + 256 + (size_t)2 * TAB_NB * 32 * 16 + 1024 + stat_bytes;   // ... + bias + stats
-  const size_t limit = 227 * 1024;
-  MCVD_CHECK(fixed + 2 * b_stage <= limit, "CONV_UMMA: tile does not fit shared memory (W=%d)", op.W);
-  int NB = (int)((limit - fixed) / b_stage);
-  if (NB > 10) NB = 10;
-  a.NB = NB;
-  const size_t smem = fixed + (size_t)NB * b_stage;
-  cudaError_t e = cudaFuncSetAttribute(k_conv_umma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit);
-  MCVD_CHECK(e == cudaSuccess, "CONV_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-  const long long tiles_m = (a.Qtot + MTOT - 1) / MTOT;
-  a.ntiles = (int)(tiles_m * a.tiles_n);
+  MCVD_CHECK(tiles_m * a.tiles_n < (1LL << 31), "%s: too many tiles", name);
+  a.ntiles = (int)(tiles_m * (a.tiles_n / a.NPI));
   const int grid = a.ntiles < sms ? a.ntiles : sms;
-  k_conv_umma<<<grid, NTHREADS, smem, s>>>(a);
-  MCVD_CUDA_LAUNCH_CHECK("conv_umma");
-  return 0;
+  switch (NT) {
+#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, p.smem, grid, s);
+    MCVD_NT_CASE(16) MCVD_NT_CASE(32) MCVD_NT_CASE(48) MCVD_NT_CASE(64) MCVD_NT_CASE(80) MCVD_NT_CASE(96)
+    MCVD_NT_CASE(112) MCVD_NT_CASE(128) MCVD_NT_CASE(144) MCVD_NT_CASE(160) MCVD_NT_CASE(176) MCVD_NT_CASE(192)
+    MCVD_NT_CASE(208) MCVD_NT_CASE(224) MCVD_NT_CASE(240) MCVD_NT_CASE(256)
+#undef MCVD_NT_CASE
+    default: break;
+  }
+  MCVD_CHECK(false, "%s: n tile %d", name, NT);
 }
+
+long long pack(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB, void* out, int scale_log2,
+               int stage_off, int per_unit, void* stream) {
+  if ((KB != 16 && KB != 32) || Cin % KB || n_tile < 16 || n_tile % 16 || Cout % n_tile) {
+    set_error("umma_pack_weights: Cin %d / Cout %d / n_tile %d / KB %d unsupported", Cin, Cout, n_tile, KB);
+    return -1;
+  }
+  const long long bytes = (long long)taps * Cin * Cout * 4;      // hi + lo fp16
+  if (!out) return bytes;
+  if (!w_taps) {
+    set_error("umma_pack_weights: null input");
+    return -1;
+  }
+  const float scale = ldexpf(1.0f, scale_log2);
+  const long long total = (long long)taps * Cin * Cout;
+  long long blocks = (total + 255) / 256;
+  if (blocks > 132LL * 16) blocks = 132LL * 16;
+  k_pack_weights<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w_taps, (__half*)out, taps, Cin, Cout, n_tile, KB,
+                                                                      scale, stage_off, per_unit);
+  if (cudaGetLastError() != cudaSuccess) {
+    set_error("umma_pack_weights: launch failed");
+    return -2;
+  }
+  return bytes;
+}
+
+}  // namespace
+
+int launch_conv_umma(const McvdOp& op, cudaStream_t s) { return launch_conv(op, s, false); }
+int launch_conv_umma2(const McvdOp& op, cudaStream_t s) { return launch_conv(op, s, true); }
 
 }  // namespace mcvd
 
@@ -753,26 +564,38 @@ extern "C" int mcvd_umma_kblock(int C0, int C1) { return mcvd::pick_kb(C0, C1); 
 
 extern "C" long long mcvd_umma_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB,
                                             void* out, int scale_log2, void* stream) {
-  if ((KB != 16 && KB != 32) || Cin % KB || n_tile < 16 || n_tile % 16 || Cout % n_tile) {
-    mcvd::set_error("umma_pack_weights: Cin %d / Cout %d / n_tile %d unsupported", Cin, Cout, n_tile);
-    return -1;
-  }
-  long long halfs = (long long)taps * Cin * Cout * 2;  // hi + lo
-  long long bytes = halfs * 2;
-  if (!out) return bytes;
-  if (!w_taps) {
-    mcvd::set_error("umma_pack_weights: null input");
-    return -1;
-  }
-  float scale = ldexpf(1.0f, scale_log2);
-  long long total = (long long)taps * Cin * Cout;
-  long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
-  mcvd::k_pack_weights<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w_taps, (__half*)out, taps, Cin, Cout,
-                                                                           n_tile, KB, scale);
-  if (cudaGetLastError() != cudaSuccess) {
-    mcvd::set_error("umma_pack_weights: launch failed");
-    return -2;
-  }
-  return bytes;
+  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, 0, KB ? (Cin / KB) * taps : 0, stream);
+}
+
+extern "C" int mcvd_umma2_plan(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats) {
+  const int kb = mcvd::conv_kb(C0, C1, C2, C3);
+  mcvd::Plan p;
+  if (!kb || n_tile < 16 || n_tile > 256 || n_tile % 16) return 0;
+  return mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, p) ? kb : 0;
+}
+
+// shared-memory plan of a conv (diagnostics / tests): out[0..9] = KB, HP, image stages, raw-ring stages (0), weight
+// stages, image slots per tile, accumulator columns outside registers (0), dynamic shared memory bytes, tiles
+// per unit (1), accumulator sets (1); returns 0, or -1
+extern "C" int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats,
+                                    int* out) {
+  const int kb = mcvd_umma2_plan(H, W, ks, C0, C1, C2, C3, n_tile, stats);
+  if (!kb || !out) return -1;
+  mcvd::Plan p;
+  mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, p);
+  out[0] = kb; out[1] = p.HP; out[2] = 2; out[3] = 0; out[4] = p.NB; out[5] = p.NJ; out[6] = 0;
+  out[7] = (int)p.smem; out[8] = 1; out[9] = 1;
+  return 0;
+}
+
+extern "C" long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cout) {
+  const long long pimg = ks == 3 ? (long long)(H + 1) * (W + 1) : (long long)H * W;
+  const long long tiles = 2 * ((B * pimg + 2 * mcvd::MT - 1) / (2 * mcvd::MT));
+  const long long nj = (mcvd::MT - 1) / pimg + 2;
+  return tiles * nj * 2 * Cout * 8;
+}
+
+extern "C" long long mcvd_umma2_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB,
+                                             void* out, int scale_log2, int stage_off, int per_unit, void* stream) {
+  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, stage_off, per_unit, stream);
 }

@@ -58,7 +58,7 @@ int launch_copy(const McvdOp& op, cudaStream_t s) {
   MCVD_CHECK(op.src0 && op.dst, "COPY: null pointer");
   long long n = (long long)op.i0 + ((long long)op.i1 << 31);
   unsigned g = (unsigned)((n + 255) / 256);
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (g == 0) g = 1;
   k_copy<<<g, 256, 0, s>>>((const float*)op.src0, (float*)op.dst, n);
   MCVD_CUDA_LAUNCH_CHECK("copy");
@@ -626,7 +626,7 @@ int launch_apply(const McvdOp& op, cudaStream_t s) {
   } else {
     long long total = (long long)op.B * op.H * op.W * ((op.C0 + op.C1) / 4);
     long long blocks = (total + 255) / 256;
-    if (blocks > 148LL * 32) blocks = 148LL * 32;
+    if (blocks > 132LL * 32) blocks = 132LL * 32;
     k_apply<<<(unsigned)blocks, 256, 0, s>>>(a);
   }
   MCVD_CUDA_LAUNCH_CHECK("apply");
@@ -655,7 +655,7 @@ int launch_resize_nearest(const McvdOp& op, cudaStream_t s) {
   MCVD_CHECK(op.src0 && op.dst, "RESIZE_NEAREST: null pointer");
   long long total = (long long)op.B * op.H * op.W * op.C0;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   k_resize_nearest<<<(unsigned)blocks, 256, 0, s>>>((const float*)op.src0, (float*)op.dst, op.B, op.i0, op.i1, op.H,
                                                     op.W, op.C0);
   MCVD_CUDA_LAUNCH_CHECK("resize_nearest");
@@ -665,7 +665,7 @@ int launch_resize_nearest(const McvdOp& op, cudaStream_t s) {
 // ------------------------------------------------------------------------------------------------
 // reverse-diffusion update (DDPM / DDIM / denoise), optional in-kernel Philox4x32-10 normal noise.
 // The Philox stream is keyed by (seed, global clip id, step, element) so a clip draws the same noise
-// whichever GPU owns it (multi-GPU equivalence, SURVEY.md section 8e).
+// whichever GPU owns it (multi-GPU equivalence).
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
                                               uint32_t k1, uint32_t out[4]) {

@@ -1,4 +1,4 @@
-// Shared helpers for the mcvd_b200 kernels (sm_100a only).
+// Shared helpers for the mcvd_b200 kernels (sm_90a).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -46,7 +46,6 @@ int launch_resize_nearest(const McvdOp& op, cudaStream_t s);
 int launch_diffusion_update(const McvdOp& op, cudaStream_t s);
 int launch_conv_umma(const McvdOp& op, cudaStream_t s);
 int launch_conv_umma2(const McvdOp& op, cudaStream_t s);
-bool try_launch_conv1x1(const McvdOp& op, cudaStream_t s, int& rc);   // conv1x1_umma.cu; false = not eligible
 int launch_conv_smalln(const McvdOp& op, cudaStream_t s);
 int launch_copy(const McvdOp& op, cudaStream_t s);
 int launch_attention_umma(const McvdOp& op, cudaStream_t s);

@@ -1,9 +1,10 @@
-// Inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by the tensor-core kernels:
-// mbarrier, 1-D bulk copy (TMA), proxy fences, TMEM allocation, tcgen05.mma / commit / ld, and the
-// shared-memory matrix descriptor (K-major, no swizzle).
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the tensor-core kernels:
+// mbarrier, 1-D bulk copy (TMA), proxy fences, warpgroup MMA (wgmma) fences / groups, and the shared-memory matrix descriptor (K-major, no swizzle).
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
+
+#include "wgmma_ops.cuh"
 
 namespace mcvd {
 namespace ptx {
@@ -36,40 +37,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// waiters that are not on the critical path (producers waiting for a free stage, epilogue warps waiting for an
-// accumulator, the weight loader): try_wait with an explicit suspend-time hint, so the warp is parked by the
-// hardware instead of spinning.  Without the hint try_wait returns almost immediately: 17 polling warps executed
-// 36 M TRYWAIT+BRA pairs in one conv launch and took a third of all issue slots -- away from the single MMA-issuing
-// warp (profiles/r2_ncu_conv2_summary.txt).
-__device__ __forceinline__ void mbar_wait_parked(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity), "r"(0x989680u)
-        : "memory");
-  } while (!done);
-}
-// non-suspending variant: mbarrier.test_wait returns at once, the thread spins (latency-critical single pollers)
-__device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
 // named barrier over a subset of the CTA's warps (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -81,149 +48,37 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- warpgroup MMA ------------------------------------------------------------------------------
+// wgmma_fence orders the warpgroup's register / shared-memory accesses before the next wgmma; commit closes a group of
+// issued wgmmas; wait<N> blocks until at most N groups are still pending (their accumulators may then be read).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t r[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// keep the compiler from moving accumulator reads / writes across an asynchronous wgmma
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// K-major, no-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
+// K-major, no-swizzle shared-memory matrix descriptor (wgmma "interleave" layout, cute::GMMA::GmmaDescriptor):
 //   [0,14) start>>4 | [16,30) LBO>>4 (K-direction core-matrix stride) | [32,46) SBO>>4 (8-row group
-//   stride) | [46,48) version = 1 | [61,64) layout = 0 (SWIZZLE_NONE)
+//   stride) | [62,64) layout = 0 (no swizzle).  A core matrix is 8 rows x 16 bytes, rows 16 bytes apart.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-
-
-// ---- thread-block clusters / CTA pairs (cta_group::2) ---------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t num_clusters_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-  return r;
-}
-// all threads of both CTAs: arrive (release) + wait (acquire)
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same offset in CTA `rank`
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier in another CTA of the cluster.  Default semantics (.release at CTA scope), as CUTLASS's
-// ClusterBarrier::arrive(cta_id) does: the data this publishes is the ARRIVING CTA's own shared memory, consumed by
-// its own tensor core.  (.release.cluster compiles to MEMBAR.ALL.GPU + ERRBAR per arrive, which also waits for the
-// thread's cp.async prefetches in flight.)
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait on a local mbarrier whose arrivals come from the peer CTA (acquire at cluster scope)
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// M = 256 across the CTA pair: each CTA supplies its own 128 rows of A and half of the N columns of B from the
-// SAME shared-memory offsets; issued by the leader CTA (rank 0) only
-__device__ __forceinline__ void umma2_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior MMAs of this thread -> arrive on the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma2_commit_mc(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"((uint16_t)3)
-      : "memory");
-}
-
-// ---- cp.async (LDGSTS): 16-byte global -> shared copies, zero-filled when src_bytes == 0 -------------
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
+// descriptor with the start-address field advanced by `units16` (16-byte units); fields do not overlap
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t units16) { return d + (uint64_t)units16; }
 
 __device__ __forceinline__ uint32_t pack_half2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
-// one elected lane of a converged warp (lets the compiler emit straight-line UTCHMMA / UBLKCP code
-// instead of a per-active-thread ELECT loop)
+// one elected lane of a converged warp
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -235,8 +90,6 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// descriptor with the start-address field advanced by `units16` (16-byte units); fields do not overlap
-__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t units16) { return d + (uint64_t)units16; }
 
 // ---- cheap math for the operand producers ------------------------------------------------------
 // SiLU with the approximate SFU ops (ex2.approx / rcp.approx, <= 2 ulp each): x / (1 + 2^(-x*log2 e))
@@ -246,8 +99,7 @@ __device__ __forceinline__ float silu_fast(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
   return x * r;
 }
-// SiLU on 8 values with the five dependent stages issued stage-by-stage (8-way ILP; written out so the
-// compiler cannot fold the chains through one temporary when registers are tight)
+// SiLU on 8 values with the five dependent stages issued stage-by-stage (8-way ILP)
 __device__ __forceinline__ void silu_fast8(float v[8]) {
   float t[8];
 #pragma unroll
@@ -261,46 +113,13 @@ __device__ __forceinline__ void silu_fast8(float v[8]) {
 #pragma unroll
   for (int e = 0; e < 8; ++e) v[e] *= t[e];
 }
-
-__device__ __forceinline__ void silu_fast4(float v[4]) {
-  float t[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) t[e] = v[e] * -1.4426950408889634f;
-#pragma unroll
-  for (int e = 0; e < 4; ++e) asm volatile("ex2.approx.ftz.f32 %0, %0;" : "+f"(t[e]));
-#pragma unroll
-  for (int e = 0; e < 4; ++e) t[e] += 1.0f;
-#pragma unroll
-  for (int e = 0; e < 4; ++e) asm volatile("rcp.approx.ftz.f32 %0, %0;" : "+f"(t[e]));
-#pragma unroll
-  for (int e = 0; e < 4; ++e) v[e] *= t[e];
-}
-// two fp32 -> fp16 hi pair + fp16 lo pair (lo = fp16(v - float(hi))); one packed convert per pair
+// two fp32 -> fp16 hi pair + fp16 lo pair (lo = fp16(v - float(hi))).  Both conversions saturate to the largest
+// finite fp16 (cvt .satfinite), so a value beyond the fp16 range degrades to a coarser finite value instead of
+// inf - inf = NaN.
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __half2 h = __floats2half2_rn(a, b);
-  const float2 hf = __half22float2(h);
-  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-
-// 256-bit global accesses (sm_100: LDG.256 / STG.256); 32-byte aligned addresses
-__device__ __forceinline__ void ldg256(const float* p, float v[8]) {
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
-}
-__device__ __forceinline__ void stg256(float* p, const float v[8]) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-               "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]));
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 [4,6)=1, a/b format F16 = 0,
-// K-major A and B (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - hf.y), "f"(a - hf.x));
 }
 
 }  // namespace ptx

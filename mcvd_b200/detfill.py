@@ -88,7 +88,7 @@ def randomize_state_dict(sd, seed: int = 1234):
 
 
 def synthetic_inputs(config, batch: int, seed: int = 1234):
-    """x_T ~ N(0,1) [B, C*F, S, S] and cond ~ U(-1,1) [B, C*Fc, S, S] (SURVEY.md section 8d)."""
+    """x_T ~ N(0,1) [B, C*F, S, S] and cond ~ U(-1,1) [B, C*Fc, S, S]."""
     C, F = config.data.channels, config.data.num_frames
     Fc = config.data.num_frames_cond + getattr(config.data, "num_frames_future", 0)
     S = config.data.image_size

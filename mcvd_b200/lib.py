@@ -177,14 +177,9 @@ def umma2_plan_info(H, W, ks, c0, c1, c2, c3, n_tile, stats):
     return dict(zip(("kb", "hp", "sa", "r", "nb", "nj", "tmem_cols", "smem", "j", "nsets"), list(out)))
 
 
-def conv1x1_enabled() -> bool:
-    """The input-stationary 1x1 kernel (csrc/conv1x1_umma.cu) is on unless MCVD_CONV1X1=0 (read by the library too)."""
-    return os.environ.get("MCVD_CONV1X1", "1") != "0"
-
-
 def umma2_pick_nt(cout: int, ks: int) -> int:
     """n tile of an OP_CONV_UMMA2 op: the largest multiple of 16 dividing Cout that is <= 128 for 3x3 convs (two or more
-    position tiles then share every weight stage, TMEM holds two accumulator sets) and <= 256 for 1x1 convs (few
+    position tiles then share every weight stage) and <= 256 for 1x1 convs (few
     weights; fewer n tiles mean fewer re-stagings of the input slab).  0 when Cout is not a multiple of 16."""
     cap = 128 if ks == 3 else 256
     best = 0

@@ -117,7 +117,7 @@ class _UNet(nn.Module):
 
 
 class UNetMore_DDPM(nn.Module):
-    """B200-native score network with the reference's module interface."""
+    """H100-native score network with the reference's module interface."""
 
     def __init__(self, config):
         super().__init__()
@@ -165,7 +165,7 @@ class UNetMore_DDPM(nn.Module):
         [B, C*Fc, S, S] or None.  ``cond_mask`` only matters for ``cond_emb=True`` nets, which are not
         built by this class (reference ncsnpp_more.py:283-287)."""
         if not x.is_cuda and not (self._engine is not None and self._engine.backend is not None):
-            raise RuntimeError("mcvd_b200.UNetMore_DDPM runs on CUDA (sm_100a) only; no CPU fallback exists")
+            raise RuntimeError("mcvd_b200.UNetMore_DDPM runs on CUDA (sm_90a) only; no CPU fallback exists")
         return self.engine().forward(x, y, cond)
 
 

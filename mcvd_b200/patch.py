@@ -1,5 +1,5 @@
 """Drop-in shim: make the UNMODIFIED reference (``main.py --config ... --video_gen``,
-``load_model_from_ckpt.py``, the demo notebook) use the B200 path.
+``load_model_from_ckpt.py``, the demo notebook) use the H100 path.
 
     import mcvd_b200.patch; mcvd_b200.patch.install()      # before NCSNRunner / load_model are used
 
@@ -49,7 +49,7 @@ def install(verbose: bool = True):
                 raise RuntimeError("mcvd_b200 module used with a sampler option the fast path does not cover "
                                    "(gamma=True); build the reference model for it")
             if is_fast and not x_mod.is_cuda and next(net.parameters()).device.type != "cuda":
-                raise RuntimeError("mcvd_b200 module on a CPU device: the fast path is CUDA (sm_100a) only and has "
+                raise RuntimeError("mcvd_b200 module on a CPU device: the fast path is CUDA (sm_90a) only and has "
                                    "no CPU fallback; build the reference model for CPU runs")
             use_fast = is_fast
             return (fast_fn if use_fast else ref_fn)(x_mod, scorenet, *a, **kw)

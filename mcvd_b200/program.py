@@ -33,7 +33,7 @@ GN_MIN_CHUNKS = 32   # ... but at least this many chunks per sample (8-pixel flo
 
 def gn_chunks(hw: int) -> int:
     """Chunks (CTAs per sample) of the GroupNorm partial pass: 64-pixel chunks on large maps, but never fewer
-    than GN_MIN_CHUNKS chunks (8-pixel floor) so the 8x8 .. 32x32 levels still put >= 512 CTAs on the 148 SMs at B = 64
+    than GN_MIN_CHUNKS chunks (8-pixel floor) so the 8x8 .. 32x32 levels still put >= 512 CTAs on the 132 SMs at B = 64
     (one chunk per sample left them latency-bound at ~22 us per launch)."""
     return max(1, min(hw // 8, max(hw // GN_PPC, GN_MIN_CHUNKS)))
 
@@ -94,7 +94,7 @@ class Engine:
     def __init__(self, module, _test_backend=None):
         """``_test_backend`` is a seam for the CPU test-suite only (tests/op_interpreter.py executes the
         lowered program so the host logic can be checked without a GPU).  Product code never passes it:
-        without it the engine requires a CUDA device and the sm_100a library, and fails loudly."""
+        without it the engine requires a CUDA device and the sm_90a library, and fails loudly."""
         self.module = module
         self.spec: arch.NetSpec = module.spec
         self.device = next(module.parameters()).device
@@ -105,20 +105,18 @@ class Engine:
                 raise RuntimeError("mcvd_b200: the module must live on a CUDA device (no CPU fallback)")
             with torch.cuda.device(self.device):
                 cc = self.lib.mcvd_device_arch()
-            if cc < 100:
-                raise RuntimeError(f"mcvd_b200 kernels are built for sm_100a only (device reports sm_{cc}: "
+            if cc != 90:
+                raise RuntimeError(f"mcvd_b200 kernels are built for sm_90a (H100) only (device reports sm_{cc}: "
                                    f"{lib.last_error()})")
-        # 'umma' (single-CTA tcgen05 kernel, default) | 'umma2' (CTA-pair cta_group::2 kernel: correct, but slower on
-        # this network's 96-channel layers -- DESIGN.md section 6) | 'simt' (CUDA cores)
+        # 'umma' (wgmma tensor-core conv, default) | 'umma2' (the same kernel fed the planar norm table, with GroupNorm
+        # statistics from the conv epilogue) | 'simt' (CUDA cores)
         self.conv_mode = os.environ.get("MCVD_CONV", "umma").lower()
         self.split_mode = int(os.environ.get("MCVD_SPLIT", "3"))            # operand split (accuracy experiments)
-        # GroupNorm partial sums from the conv epilogue instead of a k_gn_partial pass.  Measured on cfg2 (B200): the
-        # integer statistics make the 4-warp epilogue the bottleneck of the 96-channel layers (+1.0 ms of conv time,
-        # +0.5 ms in the finalize kernels) against 0.97 ms saved, so the separate pass stays the default for the
-        # round-1 kernel; the CTA-pair kernel (8 epilogue warps) always uses them.
-        # 1x1 skip projection (Conv_2): 'auto' runs it on the input-stationary 1x1 kernel (conv1x1_umma.cu) and adds
-        # the result as the residual of Conv_1 when that kernel takes it (<= 320 input channels), else rides along
-        # Conv_1 as a second K-segment; '1' always fuses (round-1 behaviour), '0' never
+        # GroupNorm partial sums from the conv epilogue instead of a k_gn_partial pass (default only with 'umma2').
+        # 1x1 skip projection (Conv_2): 'auto' / '1' ride along Conv_1 as a second K-segment wherever the K-blocks allow
+        # (one launch and one activation write + read fewer per ResBlock); '0' runs it as its own 1x1 conv added as
+        # Conv_1's residual.  cfg2, B = 64, 100 DDPM steps on an H100 80GB HBM3 (700 W): fused 105.0 frames/s,
+        # separate 104.4 frames/s.
         self.fuse_shortcut = os.environ.get("MCVD_FUSE_SC", "auto")
         self.epilogue_stats = os.environ.get("MCVD_EPISTATS", "1" if self.conv_mode == "umma2" else "0") == "1"
         self.attn_mode = os.environ.get("MCVD_ATTN", "umma").lower()        # 'umma' | 'simt'
@@ -126,7 +124,7 @@ class Engine:
         self.packed: Dict[str, object] = {}
         self.packed_version = None
         # optional on-disk cache of the packed (kernel-layout fp16 hi/lo) conv weights, keyed by a fingerprint of the
-        # checkpoint: MCVD_WEIGHT_CACHE=<dir> (SURVEY.md section 8f row 4).  Packing a 163 M-parameter checkpoint takes
+        # checkpoint: MCVD_WEIGHT_CACHE=<dir>.  Packing a 163 M-parameter checkpoint takes
         # ~0.3 s of GPU time plus one program build; the cache turns it into a file read.
         self.cache_dir = os.environ.get("MCVD_WEIGHT_CACHE") or None
         self.packs_computed = 0
@@ -278,7 +276,7 @@ class Engine:
         return torch.cat(parts, dim=1).contiguous().view(-1), float(2.0 ** (-k))
 
     def _pack_umma2(self, taps: torch.Tensor, taps_sc: Optional[torch.Tensor], nt: int, kb: int):
-        """CTA-pair weight images (conv_umma2.cu): main conv stages, then the fused 1x1 shortcut's, per n tile."""
+        """Weight images of the planar-table conv variant: main conv stages, then the fused 1x1 shortcut's, per n tile."""
         if self.backend is not None:
             flat = taps.reshape(-1) if taps_sc is None else torch.cat([taps.reshape(-1), taps_sc.reshape(-1)])
             t, _ = self.backend.pack_umma(flat.contiguous(), nt, kb)
@@ -306,7 +304,7 @@ class Engine:
     # ------------------------------------------------------------------------------ lowering
     def program(self, B: int, check_weights: bool = True) -> Program:
         """The lowered program for batch size B.  Every program owns its activation buffers (a few GB at the
-        BASELINE batch sizes), so only MAX_PROGRAMS are kept: uneven shards / last batches evict the least
+        benchmark batch sizes, mcvd_b200/configs.py), so only MAX_PROGRAMS are kept: uneven shards / last batches evict the least
         recently used one instead of piling up."""
         if B <= 0:
             raise ValueError(f"mcvd_b200: batch size {B} (an empty shard?) cannot be lowered")
@@ -428,8 +426,7 @@ class Engine:
             if shortcut is not None:                       # (Src, wname, bname): 1x1 Conv_2 of the skip branch
                 sc_src, sc_w, sc_b = shortcut
                 kb2 = lib.umma_kblock(sc_src.c0, sc_src.c1) if kb else 0
-                k1_ok = kb2 == 32 and sc_src.C <= 320 and lib.conv1x1_enabled()
-                fuse = self.fuse_shortcut == "1" or (self.fuse_shortcut == "auto" and not k1_ok)
+                fuse = self.fuse_shortcut != "0"
                 if kb and nt and kb2 and (tab is None or H >= 8) and fuse:
                     kb = min(kb, kb2)
                     sc = (sc_src, self._conv_taps(sd(sc_w)))
@@ -445,7 +442,7 @@ class Engine:
                     else:                                  # both segments share one power-of-two scale
                         self.packed[pk] = self._pack_umma_fused(taps, sc[1], nt, kb)
                 wp, wscale = self.packed[pk]
-                nacc = 0                       # auto: chosen by the launcher (TMEM double-buffering, grid fill)
+                nacc = 0                       # work organisation: the launcher's choice (input-stationary 1x1 / streaming)
                 fl = (lib.F_ACT_IN if act_in else 0) | (lib.F_ACT_OUT if act_out else 0)
                 kw2 = {}
                 if sc is not None:

@@ -2,7 +2,7 @@
 
 Restates (does not copy) ``runners/ncsn_runner.py``: ``conditioning_fn`` (:104-147), the AR loop of
 ``NCSNRunner.video_gen`` (:1501-1570) and ``get_sampler`` (:2702-2714); the dataset, metric, gif and
-checkpoint-sweep code around them is out of scope (SURVEY.md section 8).
+checkpoint-sweep code around them is out of scope.
 
 Multi-GPU: the reference wraps the network in ``torch.nn.DataParallel`` (:1377) and re-broadcasts all
 weights on every one of the 101 x n_iter network calls.  Here every clip (batch element) is
@@ -173,7 +173,7 @@ def video_gen_sharded(config, scorenet, cond_all: torch.Tensor, rank: int, world
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# evaluation of generated clips on the GPU (SURVEY.md section 8f rows 2 and 3)
+# evaluation of generated clips on the GPU
 # ---------------------------------------------------------------------------------------------------------------
 def frame_metrics(config, pred: torch.Tensor, real: torch.Tensor) -> torch.Tensor:
     """Per-frame MSE and SSIM of generated clips, on the GPU: float64 [B, frames, 2].

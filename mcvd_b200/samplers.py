@@ -249,7 +249,7 @@ def FPNDM_sampler(x_mod, scorenet, cond=None, final_only=False, denoise=True, su
     [-1] + steps[:-1], fractional mid-timesteps fed to the network, no final denoise call.  Every
     network call (L + 9 of them) runs in the CUDA library; the eps history (``ets``), its 4-term linear
     combination and the per-step ``transfer`` are a handful of tiny elementwise torch ops on the GPU
-    (fusing them into the update kernel is listed under "next" in DESIGN.md).
+    (they could be fused into the update kernel).
     """
     lp = _Loop(x_mod, scorenet, cond)
     try:

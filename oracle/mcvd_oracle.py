@@ -1,17 +1,17 @@
 """CPU oracle for the MCVD DDPM-sampling hot path.  TEST INFRASTRUCTURE ONLY.
 
 This file is a plain PyTorch fp32 *restatement* of the reference algorithm (voletiv/mcvd-pytorch
-@ 451da2e) for the path BASELINE.json names: the conditional NCSN++ ("UNetMore") score network,
+@ 451da2e) for the sampling path: the conditional NCSN++ ("UNetMore") score network,
 the DDPM / DDIM / F-PNDM reverse-diffusion loops and the autoregressive ``video_gen`` outer loop.
 It is functional (driven by a reference-format ``state_dict``), runs on the CPU, and exists so the
-CUDA path can be checked on the GPU box where ``/root/reference`` does not exist.
+CUDA path can be checked where the reference tree is not available.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl reference``
 legs may import this module.  The product package ``mcvd_b200`` never does.
 
-Pinning: the reference has NO tests or golden vectors for this path (SURVEY.md section 4/8c), so the
+Pinning: the reference has NO tests or golden vectors for this path, so the
 oracle is pinned against the reference *itself*, imported in place on the build container:
-``tests/test_host_cpu.py::test_oracle_and_module_pinned_to_live_reference`` (runs where /root/reference exists) and the committed
+``tests/test_host_cpu.py::test_oracle_and_module_pinned_to_live_reference`` (runs where the reference tree is available) and the committed
 fixtures in ``tests/golden/`` produced by ``oracle/gen_golden.py`` from the unmodified reference.
 
 Every function cites the reference file:line it restates (paths relative to the reference root).

@@ -4,8 +4,8 @@
 Follows reference ``runners/ncsn_runner.py:1581-1600`` (MSE via ``F.mse_loss``; SSIM via
 ``skimage.metrics.structural_similarity(pred_grey, real_grey, data_range=255, gaussian_weights=True,
 use_sample_covariance=False)`` on the 8-bit grey images made by ``ToPILImage()(x).convert("RGB").convert("L")``)
-and ``:2194-2196`` (best of ``preds_per_test`` repeats).  scikit-image is not installed in this image (SURVEY.md
-section 8c), so its SSIM is restated from its published algorithm (skimage/metrics/_structural_similarity.py,
+and ``:2194-2196`` (best of ``preds_per_test`` repeats).  scikit-image is not a dependency,
+so its SSIM is restated from its published algorithm (skimage/metrics/_structural_similarity.py,
 v0.19-0.24: Gaussian weights sigma = 1.5, truncate = 3.5 -> 11x11 window, ``scipy.ndimage.gaussian_filter`` with
 mode='reflect', K1 = 0.01, K2 = 0.03, population covariances, mean over the image cropped by (win - 1) // 2 = 5);
 the grey conversion is checked against PIL itself in tests/test_host_cpu.py.

@@ -1,7 +1,6 @@
 """Import the UNMODIFIED reference (voletiv/mcvd-pytorch) in place.  TEST INFRASTRUCTURE ONLY.
 
-Works only where the reference tree exists (the build container: ``/root/reference``; it does NOT
-exist on the GPU box).  Used (a) to pin ``oracle/mcvd_oracle.py`` against the real reference and
+Works only where the reference tree exists (``MCVD_REFERENCE_ROOT`` names it).  Used (a) to pin ``oracle/mcvd_oracle.py`` against the real reference and
 (b) by ``oracle/gen_golden.py`` to produce the fixtures committed under ``tests/golden/``.
 Nothing in the product package imports this.
 """
@@ -12,10 +11,10 @@ import sys
 import types
 from unittest import mock
 
-REF_ROOT = os.environ.get("MCVD_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("MCVD_REFERENCE_ROOT", "")
 
 # optional third-party modules the reference imports at module scope in runners/ncsn_runner.py
-# that are absent from this image (SURVEY.md section 8c) -- none is used on the sampling path.
+# that may be absent -- none is used on the sampling path.
 _STUBS = ["imageio", "matplotlib", "matplotlib.pyplot", "skimage", "skimage.metrics",
           "skimage.transform", "h5py", "progressbar", "seaborn", "lpips", "ninja"]
 

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_100a); run with -m gpu on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (sm_90a, H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

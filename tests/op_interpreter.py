@@ -94,7 +94,7 @@ class Interpreter:
     @staticmethod
     def _tile_geometry(B, H, W, ks):
         """(positions per image, image slots per 128-position tile, tiles) of the padded-flat position space of a
-        CONV_UMMA2 of kernel size ks (csrc/conv_umma2.cu)"""
+        CONV_UMMA2 of kernel size ks (csrc/conv_umma.cu)"""
         pimg = (H + 1) * (W + 1) if ks == 3 else H * W
         return pimg, 127 // pimg + 2, 2 * ((B * pimg + 255) // 256)
 

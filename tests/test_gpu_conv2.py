@@ -1,4 +1,4 @@
-"""CTA-pair tensor-core conv (MCVD_OP_CONV_UMMA2, csrc/conv_umma2.cu) through the C-ABI: parity against a float64
+"""Tensor-core conv with the planar norm table (MCVD_OP_CONV_UMMA2, csrc/conv_umma.cu) through the C-ABI: parity against a float64
 torch evaluation of the reference ops (nn.Conv2d / NIN after get_act_norm, models/better/layers.py:89-113,541-544,
 layerspp.py:518-549, fused Conv_2 shortcut layerspp.py:618-619), the exact integer GroupNorm statistics of its
 epilogue, and their use by MCVD_OP_GN_FINALIZE (nn.GroupNorm, layerspp.py:474-477)."""

@@ -1,8 +1,8 @@
-"""Whole-path parity on the B200 through the reference-facing API (module forward, samplers, AR loop),
+"""Whole-path parity on the H100 through the reference-facing API (module forward, samplers, AR loop),
 against the oracle (oracle/mcvd_oracle.py, pinned to the reference) and the golden fixtures generated
 from the unmodified reference (tests/golden/*.npz).
 
-Tolerances (BASELINE.json north_star): network forward rtol 1e-3 / atol 1e-4 fp32; generated frames
+Tolerances: network forward rtol 1e-3 / atol 1e-4 fp32; generated frames
 PSNR >= 50 dB on [0,1] images.
 """
 import numpy as np
@@ -19,8 +19,8 @@ RTOL, ATOL = 1e-3, 1e-4
 
 
 def gpu_module(name, conv_mode="umma"):
-    """conv_mode: simt | umma (round-1 tcgen05 kernel, GroupNorm partial pass) | umma+stats (same kernel, GroupNorm
-    partial sums from the conv epilogue) | umma2 (CTA-pair cta_group::2 kernel, epilogue statistics)"""
+    """conv_mode: simt | umma (wgmma conv kernel, GroupNorm partial pass) | umma+stats (same kernel, GroupNorm
+    partial sums from the conv epilogue) | umma2 (same kernel fed the planar norm table, epilogue statistics)"""
     cfg, net, sd = make_module(name, DEV)
     eng = net.engine()
     eng.conv_mode = conv_mode.split("+")[0]
@@ -101,7 +101,7 @@ def test_video_gen_ar_loop_vs_golden():
 
 
 def test_full_size_properties_cfg2():
-    """At BASELINE's headline size (cfg2: ngf 96, 64x64) the oracle is too slow for a CI loop, so check
+    """At the benchmark's headline size (cfg2: ngf 96, 64x64) the oracle is too slow for a CI loop, so check
     size-independent properties: (1) tensor-core path == CUDA-core fp32 path, (2) a clip's result does
     not depend on which batch it is in (what clip-sharding across GPUs relies on), (3) determinism."""
     cfg, net, sd = gpu_module("cfg2", "umma")
@@ -209,7 +209,7 @@ def test_samplers_accept_dataparallel_style_wrapper():
 
 @pytest.mark.parametrize("name", ["cfg3", "cfg4", "cfg5"])
 def test_big_configs_forward_vs_oracle(name):
-    """BASELINE.json configs[2..4] at FULL size (163 M-parameter SPADE net; ngf 192 with 192-channel heads; the 128-px
+    """Workloads cfg3..cfg5 at FULL size (163 M-parameter SPADE net; ngf 192 with 192-channel heads; the 128-px
     five-level net): one clip through the CUDA path against the oracle at two timesteps, rtol 1e-3 / atol 1e-4."""
     torch.set_num_threads(min(torch.get_num_threads(), 16))
     cfg, net, sd = gpu_module(name)
@@ -225,7 +225,7 @@ def test_big_configs_forward_vs_oracle(name):
 
 
 def test_cfg2_ten_step_sampler_vs_oracle():
-    """BASELINE.json configs[1] at full size: a 10-step DDPM sampler call (+ denoise) on one clip with injected
+    """Workload cfg2 at full size: a 10-step DDPM sampler call (+ denoise) on one clip with injected
     noise against the oracle's sampler: PSNR >= 50 dB on [0,1] frames and max |diff| < 5e-3."""
     torch.set_num_threads(min(torch.get_num_threads(), 16))
     cfg, net, sd = gpu_module("cfg2")

@@ -1,4 +1,4 @@
-"""Per-kernel parity on the B200, through the C-ABI: every op kind against a torch fp32 CPU evaluation
+"""Per-kernel parity on the H100, through the C-ABI: every op kind against a torch fp32 CPU evaluation
 of the same op (tests/op_interpreter.py semantics == include/mcvd_b200.h)."""
 import ctypes
 import math
@@ -406,7 +406,7 @@ def test_frame_metrics_vs_oracle(B, C, nf, S, rnd):
 
 
 K1_CASES = [
-    # B, H, C0, C1, Cout, tab, act_in, res, act_out      -- the input-stationary 1x1 kernel (conv1x1_umma.cu)
+    # B, H, C0, C1, Cout, tab, act_in, res, act_out      -- 1x1 convs, input-stationary and streaming (conv_umma.cu)
     (2, 16, 64, 0, 192, True, False, False, False),
     (2, 8, 96, 0, 96, False, False, True, False),
     (3, 8, 96, 96, 96, False, False, False, False),        # concatenated sources, 192 rows: a partial last tile
@@ -428,8 +428,9 @@ K1_CASES = [
 
 @pytest.mark.parametrize("case", K1_CASES)
 def test_conv1x1_stationary(case):
-    """1x1 convolutions through OP_CONV_UMMA: the input-stationary kernel against the fp64 reference, and bit-exact
-    against the general kernel (forced by asking for epilogue statistics, which the stationary kernel declines)."""
+    """1x1 convolutions through OP_CONV_UMMA in each work organisation (i2 = 2: the m tile's input resident while
+    every n tile's weights stream past; i2 = 1: one n tile per work item; i2 = 0: the launcher's choice), with and
+    without epilogue statistics: each against the fp64 reference, and all bit-identical (same K order per output)."""
     B, H, C0, C1, Cout, use_tab, act_in, use_res, act_out = case
     Cin = C0 + C1
     x0 = rnd(B, H, H, C0, seed=11)
@@ -454,14 +455,18 @@ def test_conv1x1_stationary(case):
     assert rc > 0, lib.last_error()
     fl = (lib.F_ACT_IN if act_in else 0) | (lib.F_ACT_OUT if act_out else 0)
     outs = []
-    for general in (False, True):
+    stats = []
+    for mode, with_stats in ((2, False), (1, False), (0, False), (2, True), (1, True)):
         out = torch.full((B, H, H, Cout), float("nan"), device=DEV)
         st = torch.zeros(lib.umma2_stats_bytes(B, H, H, 1, Cout) // 8, dtype=torch.int64, device=DEV) \
-            if general and H * H >= 64 else None
-        run([mk(lib.OP_CONV_UMMA, B, H=H, W=H, C0=C0, C1=C1, Cout=Cout, i0=1, i1=nt, i2=0, f0=scale, f1=2.0 ** (-k),
+            if with_stats and H * H >= 64 else None
+        run([mk(lib.OP_CONV_UMMA, B, H=H, W=H, C0=C0, C1=C1, Cout=Cout, i0=1, i1=nt, i2=mode, f0=scale, f1=2.0 ** (-k),
                 src0=x0d, src1=x1d, w=pk, bias=bd, aux0=rd, aux1=td, dst=out, dst2=st, flags=fl)])
         o = out.cpu()
         err = (o - ref).abs().max().item()
-        assert err < 2e-5 * max(1.0, ref.abs().max().item()), (case, general, err)
+        assert err < 2e-5 * max(1.0, ref.abs().max().item()), (case, mode, with_stats, err)
         outs.append(o)
-    assert torch.equal(outs[0], outs[1]), case
+        if st is not None:
+            stats.append(st.cpu())
+    assert all(torch.equal(outs[0], o) for o in outs[1:]), case
+    assert all(torch.equal(stats[0], s_) for s_ in stats[1:]), case

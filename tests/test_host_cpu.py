@@ -1,5 +1,5 @@
 """CPU-side checks (-m "not gpu"): the oracle against the committed golden vectors (and against the
-unmodified reference where /root/reference exists), the C-ABI library's exported surface, and the host
+unmodified reference where MCVD_REFERENCE_ROOT names its tree), the C-ABI library's exported surface, and the host
 logic that does not need a GPU."""
 import ctypes
 import os
@@ -11,7 +11,7 @@ import torch
 
 from common import golden, make_module, max_err, step_noise
 from mcvd_b200 import arch, configs, detfill, lib, runner
-from oracle import mcvd_oracle as O, ref_import
+from oracle import gen_golden as G, mcvd_oracle as O, ref_import
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -49,22 +49,32 @@ def test_oracle_matches_reference_golden_samplers_and_video(name):
     assert O.psnr01(vid, torch.from_numpy(g["video"])) > 60.0
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
 @pytest.mark.parametrize("name", ["tiny", "tiny_spade", "cfg1"])
 def test_oracle_and_module_pinned_to_live_reference(name):
+    """Our module's state_dict (names, shapes, re-randomised values) and the oracle's forward against the reference
+    module: as recorded in tests/golden/reference_pins.npz (oracle/gen_golden.py), and live where the tree is."""
     cfg = configs.workload(name)
-    ref = ref_import.build_reference_net(cfg)
     cfg2, mine, sd = make_module(name, "cpu")
-    rsd = ref.state_dict()
-    assert list(rsd.keys()) == list(mine.state_dict().keys())
-    assert all(rsd[k].shape == v.shape for k, v in mine.state_dict().items())
-    assert all(torch.equal(rsd[k], sd[k]) for k in rsd)
     B = cfg.bench_batch
     x, cond = detfill.synthetic_inputs(cfg, B)
-    t = torch.tensor([3, 640][:B] + [77] * max(0, B - 2))
+    t = G.pin_forward_t(B)
+    ours = O.unet_forward(cfg, sd, x, t, cond)
+    pins = golden("reference_pins")
+    msd = mine.state_dict()
+    assert list(pins[f"{name}_keys"]) == list(msd.keys())
+    assert list(pins[f"{name}_sha"]) == [G.sha(sd[k]) for k in msd]          # names, dtypes, shapes and values
+    assert list(pins[f"{name}_params"]) == [n for n, _ in mine.named_parameters()]   # what EMAHelper copies by
+    assert max_err(ours, torch.from_numpy(pins[f"{name}_forward"])) < 2e-5
+    if not ref_import.available():
+        return
+    ref = ref_import.build_reference_net(cfg)
+    rsd = ref.state_dict()
+    assert list(rsd.keys()) == list(msd.keys())
+    assert all(rsd[k].shape == v.shape for k, v in msd.items())
+    assert all(torch.equal(rsd[k], sd[k]) for k in rsd)
     with torch.no_grad():
         r = ref(x, t, cond=cond)
-    assert max_err(O.unet_forward(cfg, sd, x, t, cond), r) < 2e-5
+    assert max_err(ours, r) < 2e-5
     # EMA helper of the reference copies weights by parameter name into our module
     R = ref_import.ref_runner()
     ema = R.EMAHelper(mu=0.999)
@@ -162,44 +172,77 @@ def test_conditioning_and_shard_helpers():
     assert runner.shard_range(4, 7, 8) == (4, 4)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
-@pytest.mark.parametrize("p_cond,p_fut,sync", [(0.0, 0.0, False), (0.5, 0.0, False), (0.5, 0.5, False),
-                                               (0.5, 0.5, True), (0.0, 1.0, False), (0.3, 1.0, False)])
+@pytest.mark.parametrize("p_cond,p_fut,sync", list(G.MASK_CASES))
 def test_conditioning_masks_match_reference_draw_for_draw(p_cond, p_fut, sync):
     """Past / future masking of the paper's "general" models (reference runner:104-147): same Bernoulli draws in
-    the same order, so a seeded run of either implementation returns identical tensors."""
-    R = ref_import.ref_runner()
-    cfg = configs.workload("tiny")
-    cfg.data.num_frames_future = 2
-    cfg.data.prob_mask_sync = sync
-    n = cfg.data.num_frames_cond + cfg.data.num_frames + cfg.data.num_frames_future
-    X = detfill.normal("clips", (6, n, cfg.data.channels, 32, 32))
-    outs = []
-    for fn in (R.conditioning_fn, runner.conditioning_fn):
-        torch.manual_seed(7)
-        outs.append(fn(cfg, X, num_frames_pred=cfg.data.num_frames, prob_mask_cond=p_cond, prob_mask_future=p_fut))
-    (p0, c0, m0), (p1, c1, m1) = outs
-    assert torch.equal(p0, p1) and torch.equal(c0, c1) and c1.shape[1] == cfg.data.channels * (3 + 2)
-    assert (m0 is None and m1 is None) or torch.equal(m0, m1)
+    the same order, so a seeded run of either implementation returns identical tensors -- checked against the
+    reference's recorded outputs (tests/golden/reference_pins.npz), and live where the tree is."""
+    cfg, X = G.mask_setup(p_cond, p_fut, sync)
+    torch.manual_seed(7)
+    p1, c1, m1 = runner.conditioning_fn(cfg, X, num_frames_pred=cfg.data.num_frames, prob_mask_cond=p_cond,
+                                        prob_mask_future=p_fut)
+    assert c1.shape[1] == cfg.data.channels * (3 + 2)
+    u1 = runner.conditioning_fn(cfg, X, conditional=False)
+    assert u1[1] is None and u1[2] is None
+    pins, k = golden("reference_pins"), G.mask_key(p_cond, p_fut, sync)
+    assert G.sha(p1) == str(pins[f"{k}_pred"]) and G.sha(c1) == str(pins[f"{k}_cond"])
+    assert (m1 is None) == (f"{k}_mask" not in pins.files)
+    assert m1 is None or np.array_equal(m1.numpy(), pins[f"{k}_mask"])
     # unconditional models get every frame as the prediction target
-    u0, u1 = (fn(cfg, X, conditional=False) for fn in (R.conditioning_fn, runner.conditioning_fn))
-    assert torch.equal(u0[0], u1[0]) and u1[1] is None and u1[2] is None
-
-
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not on this box")
-def test_patch_shim_installs_and_falls_back_on_cpu():
-    """mcvd_b200.patch swaps get_model / samplers inside the unmodified reference; on a CPU config it
-    must hand back the reference module and the reference samplers' behaviour."""
+    assert G.sha(u1[0]) == str(pins[f"{k}_uncond"])
+    if not ref_import.available():
+        return
     R = ref_import.ref_runner()
-    import models as M
+    torch.manual_seed(7)
+    p0, c0, m0 = R.conditioning_fn(cfg, X, num_frames_pred=cfg.data.num_frames, prob_mask_cond=p_cond,
+                                   prob_mask_future=p_fut)
+    assert torch.equal(p0, p1) and torch.equal(c0, c1)
+    assert (m0 is None and m1 is None) or torch.equal(m0, m1)
+    assert torch.equal(R.conditioning_fn(cfg, X, conditional=False)[0], u1[0])
+
+
+def _stub_reference(tmp_path):
+    """A stand-in with the reference's module layout (runners.ncsn_runner.get_model, models.{ddpm,ddim,FPNDM}_sampler,
+    reference runners/ncsn_runner.py:180, models/__init__.py:39,103,207): its model is a CPU torch module, its
+    samplers return a recognisable function of their inputs."""
+    (tmp_path / "runners").mkdir()
+    (tmp_path / "models").mkdir()
+    (tmp_path / "runners" / "__init__.py").write_text("")
+    (tmp_path / "models" / "__init__.py").write_text(
+        "import torch\n"
+        "def ddpm_sampler(x_mod, scorenet, cond=None, **kw):\n    return (x_mod * 2 + cond.sum()).unsqueeze(0)\n"
+        "def ddim_sampler(x_mod, scorenet, **kw):\n    return 'reference ddim'\n"
+        "def FPNDM_sampler(x_mod, scorenet, **kw):\n    return 'reference fpndm'\n")
+    (tmp_path / "runners" / "ncsn_runner.py").write_text(
+        "import torch\nfrom models import ddpm_sampler, ddim_sampler, FPNDM_sampler\n"
+        "def get_model(config):\n    return torch.nn.Linear(2, 2)\n")
+
+
+def test_patch_shim_installs_and_falls_back_on_cpu(tmp_path, monkeypatch):
+    """mcvd_b200.patch swaps get_model / samplers inside the unmodified reference; on a CPU config it
+    must hand back the reference module and the reference samplers' behaviour.  Runs against the real reference
+    where MCVD_REFERENCE_ROOT names it, else against a stub with the reference's module layout."""
+    import sys
+    live = ref_import.available()
+    if live:
+        R = ref_import.ref_runner()
+        import models as M
+    else:
+        _stub_reference(tmp_path)
+        monkeypatch.syspath_prepend(str(tmp_path))
+        for m in ("runners", "runners.ncsn_runner", "models"):
+            monkeypatch.delitem(sys.modules, m, raising=False)
+        import runners.ncsn_runner as R
+        import models as M
     from mcvd_b200 import patch
     orig = (R.get_model, M.ddpm_sampler, M.ddim_sampler, M.FPNDM_sampler)
     try:
         patch.install(verbose=False)
+        assert R.get_model is not orig[0] and M.ddpm_sampler is not orig[1] and R.ddpm_sampler is M.ddpm_sampler
         cfg = configs.workload("tiny")
         cfg.device = torch.device("cpu")
         net = R.get_model(cfg)
-        assert type(net).__module__.startswith("models.better"), type(net)
+        assert type(net).__module__.startswith("models.better" if live else "torch.nn"), type(net)
         net.eval()
         x, cond = detfill.synthetic_inputs(cfg, 2)
         z = detfill.normal("z", x.shape)
@@ -208,6 +251,9 @@ def test_patch_shim_installs_and_falls_back_on_cpu():
         assert torch.equal(a, b)
     finally:
         R.get_model, M.ddpm_sampler, M.ddim_sampler, M.FPNDM_sampler = orig
+        if not live:
+            for m in ("runners", "runners.ncsn_runner", "models"):
+                sys.modules.pop(m, None)
 
 
 def test_metrics_oracle_grey_conversion_and_ssim_properties():

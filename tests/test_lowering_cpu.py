@@ -45,10 +45,9 @@ def test_forward_lowering_matches_oracle_and_golden(name, conv_mode):
 
 @pytest.mark.parametrize("mode", ["auto", "0", "1"])
 def test_skip_projection_lowering_modes(mode):
-    """Conv_2 (the 1x1 skip projection) either rides along Conv_1 as a second K-segment (MCVD_FUSE_SC=1, round 1) or is
-    its own 1x1 convolution whose output enters Conv_1 as the residual ('0'; 'auto' picks that when the
-    input-stationary kernel takes it).  Same network function either way; the unfused program has one more op per
-    ResBlock with a channel change."""
+    """Conv_2 (the 1x1 skip projection) either rides along Conv_1 as a second K-segment ('auto', the default, and '1')
+    or is its own 1x1 convolution whose output enters Conv_1 as the residual ('0').  Same network function either
+    way; the unfused program has one more op per ResBlock with a channel change."""
     from mcvd_b200 import lib
     cfg, net, sd = make_module("tiny", "cpu")
     eng = Engine(net, _test_backend=Interpreter())
@@ -61,8 +60,8 @@ def test_skip_projection_lowering_modes(mode):
     P = eng.program(B)
     fused = sum(1 for op in P.step_ops if op.kind == lib.OP_CONV_UMMA and op.src2)
     plain_1x1 = sum(1 for op in P.step_ops if op.kind == lib.OP_CONV_UMMA and op.i0 == 1)
-    assert (fused > 0) == (mode == "1")
-    if mode != "1":
+    assert (fused > 0) == (mode != "0")
+    if mode == "0":
         assert plain_1x1 > sum(1 for op in P.step_ops if op.kind in (lib.OP_ATTENTION, lib.OP_ATTENTION_UMMA)) * 2
     lib.validate_program(P.step_arr, len(P.step_ops))
 

@@ -1,4 +1,4 @@
-"""Full-size functional check of a BASELINE workload on the GPU: forward parity vs the oracle for a few clips
+"""Full-size functional check of a workload (mcvd_b200/configs.py) on the GPU: forward parity vs the oracle for a few clips
 (+ forward time).  usage: check_config.py cfg3 [batch]"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
