@@ -102,6 +102,13 @@ def workload(name: str) -> argparse.Namespace:
                    model=dict(ngf=32, ch_mult=[1, 2, 2], num_res_blocks=1, n_head_channels=32,
                               attn_resolutions=[8, 16], spade=True, spade_dim=32),
                    sampling=dict(subsample=10, num_frames_pred=5))
+    if name in ("tiny_general", "tiny_spade_general"):
+        # a "general" model (past and future masked in training, reference recipes *_pmask50_futurepast):
+        # interpolation, prediction with the future block zeroed and unconditional generation
+        cfg = workload(name[:-len("_general")])
+        cfg.workload = name
+        cfg.data.num_frames_future, cfg.data.prob_mask_cond, cfg.data.prob_mask_future = 2, 0.5, 0.5
+        return cfg
     if name == "tiny_rgb":  # 3 channels, 2 res blocks, heads > 1, odd group sizes
         return _mk(name, 3, data=dict(image_size=32, channels=3, num_frames=2, num_frames_cond=2),
                    model=dict(ngf=48, ch_mult=[1, 2, 3], num_res_blocks=2, n_head_channels=48,
@@ -116,4 +123,4 @@ def workload(name: str) -> argparse.Namespace:
 
 
 ALL_WORKLOADS = ("cfg1", "cfg2", "cfg3", "cfg4", "cfg5")
-TEST_WORKLOADS = ("tiny", "tiny_spade", "tiny_rgb", "tiny128")
+TEST_WORKLOADS = ("tiny", "tiny_spade", "tiny_rgb", "tiny128", "tiny_general", "tiny_spade_general")

@@ -1,8 +1,9 @@
 """Sampling slice of the reference runner: conditioning, the autoregressive block loop, clip sharding.
 
 Restates (does not copy) ``runners/ncsn_runner.py``: ``conditioning_fn`` (:104-147), the AR loop of
-``NCSNRunner.video_gen`` (:1501-1570) and ``get_sampler`` (:2702-2714); the dataset, metric, gif and
-checkpoint-sweep code around them is out of scope.
+``NCSNRunner.video_gen`` (:1501-1570), its three tasks -- prediction or interpolation, prediction with a
+future-frame model, unconditional generation -- chosen by the mode table of ``get_mode`` (:208-227), and
+``get_sampler`` (:2702-2714); the dataset, LPIPS / FVD, gif and checkpoint-sweep code around them is out of scope.
 
 Multi-GPU: the reference wraps the network in ``torch.nn.DataParallel`` (:1377) and re-broadcasts all
 weights on every one of the 101 x n_iter network calls.  Here every clip (batch element) is
@@ -12,8 +13,9 @@ finished frames (``gather_clips``).
 """
 from __future__ import annotations
 
+import logging
 import math
-from typing import Callable, List, Optional, Tuple
+from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 
@@ -83,7 +85,10 @@ def video_gen_clips(config, scorenet, cond: torch.Tensor, num_frames_pred: Optio
     """Autoregressive block generation for the clips in ``cond`` (reference runner:1501-1570).
 
     Each iteration samples ``num_frames`` frames, appends them, slides the conditioning window
-    ``cond <- cat(cond[:, C*F:], gen[:, C*max(0, F - Fc):])`` (:1537-1539) and draws a fresh init.
+    ``cond <- cat(cond[:, C*F:], gen[:, C*max(0, F - Fc):])`` (:1537-1539) and draws a fresh init.  With
+    ``num_frames_future = Ff > 0`` the last ``C*Ff`` channels of ``cond`` (the future block) stay where they are
+    and only the past part slides, ``cat(cond[:, C*F:-C*Ff], gen[:, C*max(0, F - Fc):], cond[:, -C*Ff:])``
+    (:1702-1708, :1872-1882), so the window keeps its width ``C*(Fc + Ff)``.
     Returns ``inverse_data_transform(pred)[:, :C*num_frames_pred]`` on the input device.
     ``init_fn(i, shape)`` supplies x_T of AR iteration i (default ``torch.randn``, :1476/:1551);
     ``noise_fn(i)`` optionally supplies the per-step noise list (parity tests).
@@ -92,6 +97,10 @@ def video_gen_clips(config, scorenet, cond: torch.Tensor, num_frames_pred: Optio
     S = config.data.image_size
     nfp = num_frames_pred if num_frames_pred is not None else config.sampling.num_frames_pred
     one_at_a_time = getattr(config.sampling, "one_frame_at_a_time", False)
+    if one_at_a_time and getattr(config.data, "num_frames_future", 0) > 0:
+        raise ValueError("one_frame_at_a_time with num_frames_future > 0 is not supported: the reference's window "
+                         "grows by C*num_frames_future channels per block there (runners/ncsn_runner.py:1699-1703)")
+    past = C * Fc                                        # channels of the window that slide; the rest is the future block
     n_iter = nfp if one_at_a_time else math.ceil(nfp / F)
     sampler = sampler or get_sampler(config)
     kw = dict(final_only=True, denoise=config.sampling.denoise,
@@ -122,7 +131,7 @@ def video_gen_clips(config, scorenet, cond: torch.Tensor, num_frames_pred: Optio
         if one_at_a_time:
             cond = torch.cat([cond[:, C:], gen[:, :C]], dim=1)
         else:
-            cond = torch.cat([cond[:, C * F:], gen[:, C * max(0, F - Fc):]], dim=1)
+            cond = torch.cat([cond[:, C * F:past], gen[:, C * max(0, F - Fc):], cond[:, past:]], dim=1)
     pred = torch.cat(preds, dim=1)[:, :C * nfp]
     return inverse_data_transform(config, pred)
 
@@ -146,29 +155,132 @@ def gather_clips(local: torch.Tensor, n_clips: int, rank: int, world: int, group
     return torch.cat(parts, dim=0)
 
 
-@torch.no_grad()
-def video_gen_sharded(config, scorenet, cond_all: torch.Tensor, rank: int, world: int, philox_seed: int = 1234,
-                      init_seed: int = 1234, **kw) -> torch.Tensor:
-    """Clip-sharded ``video_gen``: this rank generates its clips, then one all-gather.
+# ---------------------------------------------------------------------------------------------------------------
+# the reference's video_gen tasks
+# ---------------------------------------------------------------------------------------------------------------
+TASKS = ("interp", "pred", "gen")
 
-    Initial noise and per-step noise are keyed by the GLOBAL clip index so the result is independent of
-    the sharding (world size 1 == world size G, bit for bit).
+
+def tasks_for(config) -> List[str]:
+    """Tasks ``video_gen`` evaluates a model on, in the reference's order (1), (2), (3).
+
+    The mode table of ``NCSNRunner.get_mode`` (runners/ncsn_runner.py:208-227) for runs that compute metrics.
+    (1) is prediction for a model without future frames and interpolation for one with them; (2) is prediction
+    with the future block zeroed; (3) is unconditional generation.  A model trained without past masking but
+    with future frames it never masks does interpolation only; one that masks both gets all three, or (1) and
+    (3) when the masks are drawn together (``prob_mask_sync``).  A model that masks the past but never its
+    future frames has no row in the table: no tasks.
     """
-    n = cond_all.shape[0]
-    lo, hi = shard_range(n, rank, world)
-    dev = cond_all.device if cond_all.is_cuda else torch.device("cuda", torch.cuda.current_device())
-    cond = cond_all[lo:hi].to(dev)
+    condp = getattr(config.data, "prob_mask_cond", 0.0)
+    futrf = getattr(config.data, "num_frames_future", 0)
+    futrp = getattr(config.data, "prob_mask_future", 0.0)
+    if condp == 0.0:
+        if futrf == 0:
+            return ["pred"]
+        return ["interp"] if futrp == 0.0 else ["interp", "pred"]
+    if futrf == 0:
+        return ["pred", "gen"]
+    if futrp == 0.0:
+        return []
+    return ["interp", "gen"] if getattr(config.data, "prob_mask_sync", False) else ["interp", "pred", "gen"]
 
+
+def task_index(config, task: str) -> int:
+    """0, 1 or 2 for the reference's task (1), (2) or (3): interpolation, and prediction without future frames,
+    are (1); prediction with them is (2); generation is (3)."""
+    if task == "interp":
+        return 0
+    if task == "pred":
+        return 1 if getattr(config.data, "num_frames_future", 0) > 0 else 0
+    if task == "gen":
+        return 2
+    raise ValueError(f"unknown task {task!r}; expected one of {TASKS}")
+
+
+def task_seed(seed: Optional[int], index: int) -> Optional[int]:
+    """The seed task ``index`` runs with, derived from the caller's.  Task (1) keeps it, so prediction runs
+    exactly as before tasks existed; (2) and (3) move 2**40 apart, far beyond the ``7919 * n_iter`` the AR
+    loop adds to a Philox seed and the ``1009 * clip`` a per-clip x_T seed adds, so no two tasks share a noise
+    stream."""
+    return seed if seed is None or index == 0 else seed + (index << 40)
+
+
+def task_inputs(config, X: torch.Tensor, task: str, num_frames_pred: Optional[int] = None):
+    """(real frames, conditioning, frames to generate) of one task for the test batch ``X`` [B, T, C, S, S] in [0, 1].
+
+    ``conditioning_fn`` runs with the masking probabilities the reference evaluates the task with
+    (runners/ncsn_runner.py:1458-1459, 1622-1623, 1798-1799):
+      * ``interp``: past and future frames given, ``(0, 0)``.  It fills the ``num_frames`` frames between
+        them, so ``num_frames_pred`` may not exceed ``num_frames``.  Needs ``num_frames_future > 0``.
+      * ``pred``: ``(0, 0)``; with future frames ``(0, 1)``, the future block zeroed.
+        ``num_frames_pred`` defaults to ``sampling.num_frames_pred``.
+      * ``gen``: ``(1, 1)``, all conditioning zeroed.  Generates ``num_frames_cond + num_frames_pred`` frames
+        and has no real frames (``None``).
+    Real frames are in [0, 1] (``inverse_data_transform``); the conditioning is in the model's range.
+    """
+    C, F, Fc = config.data.channels, config.data.num_frames, config.data.num_frames_cond
+    Ff = getattr(config.data, "num_frames_future", 0)
+    nfp = num_frames_pred if num_frames_pred is not None else config.sampling.num_frames_pred
+    if task == "interp":
+        if Ff == 0:
+            raise ValueError("task 'interp' needs a model with data.num_frames_future > 0")
+        nfp = num_frames_pred if num_frames_pred is not None else F
+        if nfp > F:
+            raise ValueError(f"task 'interp' fills the {F} frames between past and future; "
+                             f"num_frames_pred={nfp} is more")
+        probs = (0.0, 0.0)
+    elif task == "pred":
+        probs = (0.0, 1.0 if Ff > 0 else 0.0)
+    elif task == "gen":
+        nfp = Fc + nfp
+        probs = (1.0, 1.0)
+    else:
+        raise ValueError(f"unknown task {task!r}; expected one of {TASKS}")
+    real, cond, _ = conditioning_fn(config, data_transform(config, X), num_frames_pred=nfp,
+                                    prob_mask_cond=probs[0], prob_mask_future=probs[1])
+    if cond.shape[1] != C * (Fc + Ff):
+        raise ValueError(f"X has {X.shape[1]} frames, too few for the {Fc} past + {F} generated + {Ff} future "
+                         "frames of the conditioning window")
+    return (None if task == "gen" else inverse_data_transform(config, real)), cond, nfp
+
+
+def clip_init_fn(init_seed: int, lo: int, hi: int, dev) -> Callable[[int, Tuple[int, ...]], torch.Tensor]:
+    """``init_fn`` for ``video_gen_clips`` over the global clips [lo, hi): one CPU generator per clip and AR
+    iteration, so clip g of AR iteration i sees the same x_T in any batch and on any GPU."""
     def init_fn(i, shape):
-        # per-clip generators: clip g of AR iteration i always sees the same x_T
         outs = []
         for g in range(lo, hi):
             gen = torch.Generator(device="cpu")
             gen.manual_seed(init_seed * 1000003 + g * 1009 + i)
             outs.append(torch.randn(shape[1:], generator=gen))
         return torch.stack(outs).to(dev) if outs else torch.empty((0,) + tuple(shape[1:]), device=dev)
+    return init_fn
 
-    local = video_gen_clips(config, scorenet, cond, init_fn=init_fn, clip_offset=lo, philox_seed=philox_seed, **kw)
+
+@torch.no_grad()
+def video_gen_sharded(config, scorenet, cond_all: torch.Tensor, rank: int, world: int, philox_seed: int = 1234,
+                      init_seed: int = 1234, task: Optional[str] = None, **kw) -> torch.Tensor:
+    """Clip-sharded ``video_gen``: this rank generates its clips, then one all-gather.
+
+    Initial noise and per-step noise are keyed by the GLOBAL clip index so the result is independent of
+    the sharding (world size 1 == world size G, bit for bit).
+
+    With a ``task`` ("interp", "pred" or "gen"), ``cond_all`` is the test batch ``X`` [B, T, C, S, S] in [0, 1]
+    instead: each rank builds the task's conditioning for its clips (``task_inputs``; ``num_frames_pred`` in
+    ``kw`` is passed on to it) and runs with the task's seeds (``task_seed``), so the guarantee holds per task.
+    """
+    n = cond_all.shape[0]
+    lo, hi = shard_range(n, rank, world)
+    dev = cond_all.device if cond_all.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    if task is None:
+        cond = cond_all[lo:hi].to(dev)
+    else:
+        _, cond, kw["num_frames_pred"] = task_inputs(config, cond_all[lo:hi], task, kw.get("num_frames_pred"))
+        cond = cond.to(dev)
+        k = task_index(config, task)
+        philox_seed, init_seed = task_seed(philox_seed, k), task_seed(init_seed, k)
+    local = video_gen_clips(config, scorenet, cond, init_fn=clip_init_fn(init_seed, lo, hi, dev), clip_offset=lo,
+                            philox_seed=philox_seed, **kw)
     return gather_clips(local, n, rank, world)
 
 
@@ -212,20 +324,55 @@ def best_of_repeats(per_frame: torch.Tensor, preds_per_test: int):
 
 
 @torch.no_grad()
+def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[int] = None,
+                   tasks: Optional[List[str]] = None, num_frames_pred: Optional[int] = None,
+                   **gen_kw) -> Dict[str, Tuple[torch.Tensor, Optional[dict]]]:
+    """One test batch of the reference's ``video_gen`` (runners/ncsn_runner.py:1392-1395, 1444-1915), every task.
+
+    ``X`` is [B, T, C, S, S] in [0, 1].  Every test clip is repeated ``preds_per_test`` times (``repeat_interleave``,
+    the reference's collate function), and each repeat is sampled with its own noise.  ``tasks`` defaults to
+    ``tasks_for(config)``; ``num_frames_pred`` applies to ``pred`` and ``gen`` (``interp`` always fills
+    ``num_frames``).  Returns ``{task: (frames [B*p, C*nfp, S, S] in [0, 1], metrics)}``.  ``metrics`` holds
+    per-clip ``mse`` / ``psnr`` / ``ssim`` of the best repeat and the ``per_frame`` values, or is ``None`` for
+    ``gen``, which has no ground truth, and for a task that predicts past the real frames of ``X`` (:1573-1579).
+
+    ``gen_kw`` go to ``video_gen_clips``.  A ``philox_seed`` among them is replaced by the task's
+    (``task_seed``).  An ``init_seed`` draws x_T per global clip (``clip_init_fn``, clips numbered from
+    ``clip_offset``) from the task's seed.  ``init_fn`` and ``noise_fn`` reach every task unchanged.
+    """
+    p = preds_per_test if preds_per_test is not None else getattr(config.sampling, "preds_per_test", 1)
+    X = X.repeat_interleave(p, dim=0)
+    dev = next(scorenet.parameters()).device
+    init_seed = gen_kw.pop("init_seed", None)
+    out = {}
+    for task in (tasks_for(config) if tasks is None else tasks):
+        real, cond, nfp = task_inputs(config, X, task, None if task == "interp" else num_frames_pred)
+        k = task_index(config, task)
+        kw = dict(gen_kw)
+        if kw.get("philox_seed") is not None:
+            kw["philox_seed"] = task_seed(kw["philox_seed"], k)
+        if init_seed is not None:
+            lo = kw.get("clip_offset", 0)
+            kw["init_fn"] = clip_init_fn(task_seed(init_seed, k), lo, lo + X.shape[0], dev)
+        frames = video_gen_clips(config, scorenet, cond.to(dev), nfp, **kw)
+        metrics = None
+        if real is not None and real.shape[1] < frames.shape[1]:
+            logging.warning("evaluate_tasks: task %r generates %d frames but X holds only %d after the conditioning "
+                            "frames; no metrics", task, nfp, real.shape[1] // config.data.channels)
+        elif real is not None:
+            per_frame = frame_metrics(config, frames, real.to(dev))
+            mse, psnr, ssim = best_of_repeats(per_frame, p)
+            metrics = {"mse": mse, "psnr": psnr, "ssim": ssim, "per_frame": per_frame}
+        out[task] = (frames, metrics)
+    return out
+
+
+@torch.no_grad()
 def evaluate_clips(config, scorenet, X: torch.Tensor, preds_per_test: Optional[int] = None,
                    num_frames_pred: Optional[int] = None, **gen_kw):
-    """One test batch of the reference's ``video_gen`` (runners/ncsn_runner.py:1392-1395, 1463-1470, 1501-1609): every
-    test clip is repeated ``preds_per_test`` times (``repeat_interleave``, the reference's collate function), each
-    repeat is sampled with its own noise, and the per-clip metrics keep the best repeat.  ``X`` is [B, T, C, S, S] in
-    [0, 1].  Returns (frames [B*p, C*nfp, S, S] in [0, 1], dict of per-clip mse / psnr / ssim tensors)."""
-    p = preds_per_test if preds_per_test is not None else getattr(config.sampling, "preds_per_test", 1)
-    nfp = num_frames_pred if num_frames_pred is not None else config.sampling.num_frames_pred
-    X = X.repeat_interleave(p, dim=0)
-    real, cond, _ = conditioning_fn(config, data_transform(config, X), num_frames_pred=nfp,
-                                    prob_mask_cond=getattr(config.data, "prob_mask_cond", 0.0))
-    dev = next(scorenet.parameters()).device
-    frames = video_gen_clips(config, scorenet, cond.to(dev), nfp, **gen_kw)
-    real01 = inverse_data_transform(config, real.to(dev))
-    per_frame = frame_metrics(config, frames, real01)
-    mse, psnr, ssim = best_of_repeats(per_frame, p)
-    return frames, {"mse": mse, "psnr": psnr, "ssim": ssim, "per_frame": per_frame}
+    """Task (1) of ``evaluate_tasks``: prediction, or interpolation for a model with future frames, with no
+    conditioning masked (runners/ncsn_runner.py:1458-1459).  ``X`` is [B, T, C, S, S] in [0, 1].  Returns
+    (frames [B*p, C*nfp, S, S] in [0, 1], dict of per-clip mse / psnr / ssim tensors and ``per_frame``)."""
+    task = "interp" if getattr(config.data, "num_frames_future", 0) > 0 else "pred"
+    return evaluate_tasks(config, scorenet, X, preds_per_test, tasks=[task], num_frames_pred=num_frames_pred,
+                          **gen_kw)[task]
