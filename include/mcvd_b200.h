@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define MCVD_ABI_VERSION 4
+#define MCVD_ABI_VERSION 5
 
 /* ---- op kinds ------------------------------------------------------------------------------- */
 enum {
@@ -91,7 +91,10 @@ enum {
    *   x0 = f0 * (x - f1 * eps);  if MCVD_F_CLIP: x0 = clamp(x0,-1,1);
    *   x  = f2 * x0 + f3 * x + f4 * eps + f5 * z
    * dst = x [B,C0,H,W] NCHW (in place); src0 = eps [B,H,W,C0] NHWC (channel pitch Cout if > 0); src1 = z NCHW or NULL
-   * (MCVD_F_PHILOX: z from Philox4x32-10 keyed by (seed=i0|i1<<32, clip id = i2 + b, step = i3)). */
+   * (MCVD_F_PHILOX: z from Philox4x32-10 keyed by (seed=i0|i1<<32, clip id = i2 + b, step = i3)).
+   * MCVD_F_GAMMA (with MCVD_F_PHILOX): z = f7 * (G - f6), G ~ Gamma(shape f6, scale 1) drawn in-kernel
+   * (Marsaglia-Tsang in fp64, mcvd_b200/csrc/elementwise.cu), i.e. the centred Gamma noise of a model trained
+   * with model.gamma=True (models/__init__.py:319-322: f6 = k_cum, f7 = theta / sqrt(1 - alpha)). */
   MCVD_OP_DIFFUSION_UPDATE = 11,
   /* 3x3 / 1x1 convolution on the Hopper tensor cores (wgmma m64nNk16 f16, fp16 hi/lo split of
    * both operands, fp32 accumulation in registers), with the GroupNorm/FiLM/SiLU transform of the input
@@ -144,6 +147,11 @@ enum {
    * 7471 B + 32768) >> 16), i.e. 11x11 Gaussian (sigma 1.5) moments, mean over the interior cropped by 5 pixels.
    * MCVD_F_ROUND: round the [0,1] values first (the reference does for (Stochastic)MovingMNIST, :1596-1599). */
   MCVD_OP_FRAME_METRICS = 17,
+  /* dst[b, c, y, x] = f5 * z for [B, C0, H, W] fp32 NCHW, z keyed exactly as in MCVD_OP_DIFFUSION_UPDATE with
+   * MCVD_F_PHILOX (seed i0|i1<<32, clip id i2 + b, step tag i3): the Philox normal, or with MCVD_F_GAMMA the
+   * centred Gamma draw f7 * (G - f6).  x_T of a Gamma-noise model (runners/ncsn_runner.py:1471-1474, 1546-1549)
+   * without a host tensor.  src0 is not read. */
+  MCVD_OP_NOISE = 18,
   MCVD_OP__COUNT
 };
 
@@ -156,6 +164,7 @@ enum {
 #define MCVD_F_CLIP     (1 << 5)   /* DIFFUSION_UPDATE: clamp x0 to [-1, 1]                        */
 #define MCVD_F_PHILOX   (1 << 6)   /* DIFFUSION_UPDATE: draw z in-kernel                           */
 #define MCVD_F_ROUND    (1 << 7)   /* FRAME_METRICS: round the images before the grey conversion   */
+#define MCVD_F_GAMMA    (1 << 8)   /* DIFFUSION_UPDATE (with PHILOX), NOISE: centred Gamma(f6) * f7 */
 
 typedef struct McvdOp {
   int32_t kind;

@@ -109,6 +109,11 @@ def workload(name: str) -> argparse.Namespace:
         cfg.workload = name
         cfg.data.num_frames_future, cfg.data.prob_mask_cond, cfg.data.prob_mask_future = 2, 0.5, 0.5
         return cfg
+    if name == "tiny_gamma":  # tiny trained with Gamma noise (model.gamma=True, Nachmani et al. 2021)
+        cfg = workload("tiny")
+        cfg.workload = name
+        cfg.model.gamma = True
+        return cfg
     if name == "tiny_rgb":  # 3 channels, 2 res blocks, heads > 1, odd group sizes
         return _mk(name, 3, data=dict(image_size=32, channels=3, num_frames=2, num_frames_cond=2),
                    model=dict(ngf=48, ch_mult=[1, 2, 3], num_res_blocks=2, n_head_channels=48,
@@ -123,4 +128,4 @@ def workload(name: str) -> argparse.Namespace:
 
 
 ALL_WORKLOADS = ("cfg1", "cfg2", "cfg3", "cfg4", "cfg5")
-TEST_WORKLOADS = ("tiny", "tiny_spade", "tiny_rgb", "tiny128", "tiny_general", "tiny_spade_general")
+TEST_WORKLOADS = ("tiny", "tiny_spade", "tiny_rgb", "tiny128", "tiny_general", "tiny_spade_general", "tiny_gamma")

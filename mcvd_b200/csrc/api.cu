@@ -34,6 +34,7 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_COPY: return launch_copy(op, s);
     case MCVD_OP_ATTENTION_UMMA: return launch_attention_umma(op, s);
     case MCVD_OP_FRAME_METRICS: return launch_frame_metrics(op, s);
+    case MCVD_OP_NOISE: return launch_noise(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -54,7 +55,7 @@ static int validate_one(const McvdOp& op, int idx) {
     set_error("op %d (kind %d): spatial size %dx%d", idx, op.kind, op.H, op.W);
     return -1;
   }
-  if (!op.src0 || !op.dst) {
+  if (!op.dst || (!op.src0 && op.kind != MCVD_OP_NOISE)) {
     set_error("op %d (kind %d): null src0/dst", idx, op.kind);
     return -1;
   }
@@ -92,6 +93,19 @@ static int validate_one(const McvdOp& op, int idx) {
       if (op.kind == MCVD_OP_ATTENTION_UMMA && (!op.dst2 || (reinterpret_cast<uintptr_t>(op.dst2) & 15))) {
         set_error("op %d ATTENTION_UMMA: dst2 (operand-image scratch) is null or not 16-byte aligned", idx);
         return -1;
+      }
+      break;
+    case MCVD_OP_DIFFUSION_UPDATE:
+    case MCVD_OP_NOISE:
+      if (op.flags & MCVD_F_GAMMA) {
+        if (op.kind == MCVD_OP_DIFFUSION_UPDATE && !(op.flags & MCVD_F_PHILOX)) {
+          set_error("op %d DIFFUSION_UPDATE: MCVD_F_GAMMA needs MCVD_F_PHILOX", idx);
+          return -1;
+        }
+        if (const char* why = gamma_params_error(op)) {
+          set_error("op %d (kind %d): %s", idx, op.kind, why);
+          return -1;
+        }
       }
       break;
     default: break;

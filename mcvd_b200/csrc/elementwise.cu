@@ -1,6 +1,8 @@
 // Memory-bound kernels of the MCVD sampling path: layout changes, timestep embedding, FiLM linears,
 // GroupNorm statistics, the fused normalise/FiLM/SPADE/SiLU/FIR "apply" pass, nearest resize and
 // the reverse-diffusion update.  All tensors fp32; activations NHWC.
+#include <cmath>
+
 #include "mcvd_common.cuh"
 
 namespace mcvd {
@@ -663,7 +665,7 @@ int launch_resize_nearest(const McvdOp& op, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// reverse-diffusion update (DDPM / DDIM / denoise), optional in-kernel Philox4x32-10 normal noise.
+// reverse-diffusion update (DDPM / DDIM / denoise), optional in-kernel Philox4x32-10 normal or Gamma noise.
 // The Philox stream is keyed by (seed, global clip id, step, element) so a clip draws the same noise
 // whichever GPU owns it (multi-GPU equivalence).
 // ------------------------------------------------------------------------------------------------
@@ -693,9 +695,46 @@ __device__ __forceinline__ float philox_normal(uint32_t seed_lo, uint32_t seed_h
   return rad * cospif(2.0f * u2);
 }
 
+// Gamma(k, 1) - k from the same Philox stream (Marsaglia & Tsang 2000, "A simple method for generating gamma
+// variables"): d = k - 1/3, c = 1/sqrt(9d), x ~ N(0,1), v = (1 + cx)^3, accept when log u < x^2/2 + d - dv + d log v.
+// Attempt a is one Philox call with counter (element, clip, step, MCVD_GAMMA_TAG | a): words 0 and 1 feed Box-Muller,
+// word 2 is u, word 3 the boost uniform for k < 1 (G(k) = G(k+1) * U^(1/k)).  Acceptance is >= 0.95 for every
+// d >= 2/3, so MCVD_GAMMA_ATTEMPTS = 16 rejections in a row happen with probability < 1e-20 per element; if they do,
+// the element takes the proposal's centre v = 1 (x = 0), i.e. G = d.
+// k reaches 2.5e10 on the linear schedule, so G - k is never formed as a difference of two large numbers:
+// with w = v - 1 = cx(3 + 3cx + c^2x^2), G - k = d w - 1/3 for k >= 1.  Everything runs in fp64; the caller
+// rounds to fp32 once.  oracle/gamma_oracle.py restates this function in numpy for the tests.
+#define MCVD_GAMMA_TAG 0x47414d00u      /* 'GAM\0' | attempt; distinct from the normal stream's 'MCVD' */
+#define MCVD_GAMMA_ATTEMPTS 16
+
+__device__ __noinline__ double philox_gamma_centred(double k, uint32_t seed_lo, uint32_t seed_hi, uint32_t clip,
+                                                    uint32_t step, uint32_t elem) {
+  const bool boost = k < 1.0;
+  const double kk = boost ? k + 1.0 : k;
+  const double d = kk - 1.0 / 3.0, c = 1.0 / sqrt(9.0 * d);
+  double w = 0.0, ub = 0.5;
+  for (int a = 0; a < MCVD_GAMMA_ATTEMPTS; ++a) {
+    uint32_t r[4];
+    philox4x32_10(elem, clip, step, MCVD_GAMMA_TAG | (uint32_t)a, seed_lo, seed_hi, r);
+    const double u1 = ((double)r[0] + 1.0) * 2.3283064365386963e-10;     // (0, 1]
+    const double u2 = ((double)r[1] + 0.5) * 2.3283064365386963e-10;
+    const double x = sqrt(-2.0 * log(u1)) * cospi(2.0 * u2);
+    const double cx = c * x;
+    ub = ((double)r[3] + 0.5) * 2.3283064365386963e-10;
+    if (cx <= -1.0) continue;                                              // v <= 0
+    const double wc = cx * (3.0 + cx * (3.0 + cx));
+    const double u = ((double)r[2] + 0.5) * 2.3283064365386963e-10;
+    if (log(u) < 0.5 * x * x + d * (log1p(wc) - wc)) { w = wc; break; }
+  }
+  if (!boost) return d * w - 1.0 / 3.0;
+  return d * (1.0 + w) * exp(log(ub) / k) - k;
+}
+
+template <bool GAMMA>
 __global__ void k_diffusion_update(float* __restrict__ x, const float* __restrict__ eps, const float* __restrict__ z,
                                    int B, int C, int HW, int pitch, float k0, float k1, float ca, float cb, float cc,
-                                   float sigma, int flags, uint32_t seed_lo, uint32_t seed_hi, int clip0, int step) {
+                                   float sigma, int flags, uint32_t seed_lo, uint32_t seed_hi, int clip0, int step,
+                                   float gk, float gscale) {
   long long total = (long long)B * C * HW;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -710,22 +749,74 @@ __global__ void k_diffusion_update(float* __restrict__ x, const float* __restric
   if (cc != 0.f) r += cc * ev;
   if (sigma != 0.f) {
     float zv;
-    if (flags & MCVD_F_PHILOX) zv = philox_normal(seed_lo, seed_hi, (uint32_t)(clip0 + b), (uint32_t)step, (uint32_t)(c * HW + p));
+    if (GAMMA)
+      zv = (float)((double)gscale * philox_gamma_centred((double)gk, seed_lo, seed_hi, (uint32_t)(clip0 + b),
+                                                         (uint32_t)step, (uint32_t)(c * HW + p)));
+    else if (flags & MCVD_F_PHILOX) zv = philox_normal(seed_lo, seed_hi, (uint32_t)(clip0 + b), (uint32_t)step, (uint32_t)(c * HW + p));
     else zv = z[i];
     r += sigma * zv;
   }
   x[i] = r;
 }
 
+// host checks of the Gamma parameters (f6 = shape k, f7 = scale) shared by the launchers and mcvd_validate_program
+const char* gamma_params_error(const McvdOp& op) {
+  if (!(op.f6 > 0.f) || !std::isfinite(op.f6)) return "Gamma shape f6 must be finite and > 0";
+  if (!std::isfinite(op.f7)) return "Gamma scale f7 must be finite";
+  return nullptr;
+}
+
 int launch_diffusion_update(const McvdOp& op, cudaStream_t s) {
   MCVD_CHECK(op.src0 && op.dst, "DIFFUSION_UPDATE: null pointer");
   MCVD_CHECK(op.f5 == 0.f || (op.flags & MCVD_F_PHILOX) || op.src1, "DIFFUSION_UPDATE: sigma != 0 needs noise");
+  const bool gamma = (op.flags & MCVD_F_GAMMA) != 0;
+  if (gamma) {
+    MCVD_CHECK(op.flags & MCVD_F_PHILOX, "DIFFUSION_UPDATE: MCVD_F_GAMMA needs MCVD_F_PHILOX");
+    const char* why = gamma_params_error(op);
+    MCVD_CHECK(!why, "DIFFUSION_UPDATE: %s", why);
+  }
   long long total = (long long)op.B * op.C0 * op.H * op.W;
-  k_diffusion_update<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+  auto kern = gamma ? k_diffusion_update<true> : k_diffusion_update<false>;
+  kern<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
       (float*)op.dst, (const float*)op.src0, (const float*)op.src1, op.B, op.C0, op.H * op.W,
       op.Cout > 0 ? op.Cout : op.C0, op.f0, op.f1, op.f2,
-      op.f3, op.f4, op.f5, op.flags, (uint32_t)op.i0, (uint32_t)op.i1, op.i2, op.i3);
+      op.f3, op.f4, op.f5, op.flags, (uint32_t)op.i0, (uint32_t)op.i1, op.i2, op.i3, op.f6, op.f7);
   MCVD_CUDA_LAUNCH_CHECK("diffusion_update");
+  return 0;
+}
+
+// dst[b, c, p] = f5 * z, z keyed exactly as in DIFFUSION_UPDATE: the Philox normal, or with MCVD_F_GAMMA the
+// centred Gamma draw of shape f6 and scale f7.  x_T of a Gamma-noise model without a host tensor.
+template <bool GAMMA>
+__global__ void k_noise(float* __restrict__ dst, int B, int C, int HW, float scale, uint32_t seed_lo,
+                        uint32_t seed_hi, int clip0, int step, float gk, float gscale) {
+  long long total = (long long)B * C * HW;
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  int p = (int)(i % HW);
+  int c = (int)((i / HW) % C);
+  int b = (int)(i / ((long long)HW * C));
+  float zv;
+  if (GAMMA)
+    zv = (float)((double)gscale * philox_gamma_centred((double)gk, seed_lo, seed_hi, (uint32_t)(clip0 + b),
+                                                       (uint32_t)step, (uint32_t)(c * HW + p)));
+  else zv = philox_normal(seed_lo, seed_hi, (uint32_t)(clip0 + b), (uint32_t)step, (uint32_t)(c * HW + p));
+  dst[i] = scale * zv;
+}
+
+int launch_noise(const McvdOp& op, cudaStream_t s) {
+  MCVD_CHECK(op.dst, "NOISE: null destination");
+  const bool gamma = (op.flags & MCVD_F_GAMMA) != 0;
+  if (gamma) {
+    const char* why = gamma_params_error(op);
+    MCVD_CHECK(!why, "NOISE: %s", why);
+  }
+  long long total = (long long)op.B * op.C0 * op.H * op.W;
+  if (total <= 0) return 0;
+  auto kern = gamma ? k_noise<true> : k_noise<false>;
+  kern<<<(unsigned)((total + 255) / 256), 256, 0, s>>>((float*)op.dst, op.B, op.C0, op.H * op.W, op.f5,
+                                                       (uint32_t)op.i0, (uint32_t)op.i1, op.i2, op.i3, op.f6, op.f7);
+  MCVD_CUDA_LAUNCH_CHECK("noise");
   return 0;
 }
 

@@ -50,5 +50,9 @@ int launch_conv_smalln(const McvdOp& op, cudaStream_t s);
 int launch_copy(const McvdOp& op, cudaStream_t s);
 int launch_attention_umma(const McvdOp& op, cudaStream_t s);
 int launch_frame_metrics(const McvdOp& op, cudaStream_t s);
+int launch_noise(const McvdOp& op, cudaStream_t s);
+
+// NULL, or why the Gamma parameters (f6 = shape, f7 = scale) of an op with MCVD_F_GAMMA are unusable
+const char* gamma_params_error(const McvdOp& op);
 
 }  // namespace mcvd

@@ -2,8 +2,8 @@
 
 Same constructor argument (the config Namespace), same ``forward(x, y, cond=None, cond_mask=None)``,
 same ``state_dict`` keys and shapes (``unet.all_modules.{i}...``, buffers ``betas / alphas /
-alphas_prev / unet.sigmas``) so reference checkpoints load with ``load_state_dict`` and
-``EMAHelper.ema`` can copy weights in by name (``models/ema.py:23-28``).  The modules below hold
+alphas_prev / unet.sigmas``, and ``k / k_cum / theta_t`` for ``model.gamma``) so reference checkpoints load
+with ``load_state_dict`` and ``EMAHelper.ema`` can copy weights in by name (``models/ema.py:23-28``).  The modules below hold
 parameters only; all arithmetic runs in the CUDA library through a lowered op program
 (``mcvd_b200/program.py``).  There is no PyTorch or CPU fallback: calling ``forward`` without the
 library or off-GPU raises.
@@ -135,7 +135,14 @@ class UNetMore_DDPM(nn.Module):
         self.register_buffer("alphas", alphas)
         self.register_buffer("alphas_prev", torch.cat([alphas[1:], torch.tensor([1.0])]))
         self.schedule = "linear"
-        self.gamma = False
+        self.gamma = bool(getattr(m, "gamma", False))
+        if self.gamma:
+            # Gamma noise (ncsnpp_more.py:743-748): per-level shape k, its cumulative sum k_cum and the scale theta_t,
+            # same names, order and fp32 expressions, so a reference gamma checkpoint loads with strict=True
+            self.theta_0 = 0.001
+            self.register_buffer("k", self.betas / (self.alphas * (self.theta_0 ** 2)))
+            self.register_buffer("k_cum", torch.cumsum(self.k.flip(0), 0).flip(0))
+            self.register_buffer("theta_t", torch.sqrt(self.alphas) * self.theta_0)
         self.noise_in_cond = False
         self.type = getattr(config.model, "type", "v1")
         self._engine = None

@@ -19,6 +19,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 
+from . import samplers
 from .samplers import get_sampler
 
 
@@ -90,7 +91,9 @@ def video_gen_clips(config, scorenet, cond: torch.Tensor, num_frames_pred: Optio
     and only the past part slides, ``cat(cond[:, C*F:-C*Ff], gen[:, C*max(0, F - Fc):], cond[:, -C*Ff:])``
     (:1702-1708, :1872-1882), so the window keeps its width ``C*(Fc + Ff)``.
     Returns ``inverse_data_transform(pred)[:, :C*num_frames_pred]`` on the input device.
-    ``init_fn(i, shape)`` supplies x_T of AR iteration i (default ``torch.randn``, :1476/:1551);
+    ``init_fn(i, shape)`` supplies x_T of AR iteration i (default ``torch.randn``, :1476/:1551; for a Gamma-noise
+    model ``Gamma(k_cum[0], scale theta_t[0]) - k_cum[0] theta_t[0]``, :1471-1474/:1546-1549, drawn on the GPU with
+    one torch-drawn seed per call, keyed by global clip and AR iteration);
     ``noise_fn(i)`` optionally supplies the per-step noise list (parity tests).
     """
     C, F, Fc = config.data.channels, config.data.num_frames, config.data.num_frames_cond
@@ -112,6 +115,9 @@ def video_gen_clips(config, scorenet, cond: torch.Tensor, num_frames_pred: Optio
     shape = (B, C * F, S, S)
     preds = []
     warm = (getattr(config.sampling, "init_prev_t", -1) or -1) > 0
+    if init_fn is None and getattr(config.model, "gamma", False):
+        init_fn = clip_init_fn(samplers.draw_seed(), clip_offset, clip_offset + B, cond.device,
+                               gamma=gamma_init_params(config, scorenet))
     gen = None
     for i in range(n_iter):
         if warm and i > 0:
@@ -244,9 +250,29 @@ def task_inputs(config, X: torch.Tensor, task: str, num_frames_pred: Optional[in
     return (None if task == "gen" else inverse_data_transform(config, real)), cond, nfp
 
 
-def clip_init_fn(init_seed: int, lo: int, hi: int, dev) -> Callable[[int, Tuple[int, ...]], torch.Tensor]:
+def gamma_init_params(config, scorenet) -> Optional[Tuple[float, float]]:
+    """(k_cum[0], theta_t[0]) of a Gamma-noise model, whose x_T is Gamma(k_cum[0], scale theta_t[0]) - k_cum[0] theta_t[0]
+    (runners/ncsn_runner.py:1471-1474); None for a model with normal noise."""
+    if not getattr(config.model, "gamma", False):
+        return None
+    net = scorenet.module if hasattr(scorenet, "module") else scorenet
+    return float(net.k_cum[0]), float(net.theta_t[0])
+
+
+def clip_init_fn(init_seed: int, lo: int, hi: int, dev,
+                 gamma: Optional[Tuple[float, float]] = None) -> Callable[[int, Tuple[int, ...]], torch.Tensor]:
     """``init_fn`` for ``video_gen_clips`` over the global clips [lo, hi): one CPU generator per clip and AR
-    iteration, so clip g of AR iteration i sees the same x_T in any batch and on any GPU."""
+    iteration, so clip g of AR iteration i sees the same x_T in any batch and on any GPU.
+
+    ``gamma = (k, theta)`` (``gamma_init_params``): x_T is the centred Gamma draw ``G - k theta``, G ~ Gamma(k, scale
+    theta), made on the GPU by ``MCVD_OP_NOISE`` from the Philox stream keyed by (init_seed, global clip, AR
+    iteration): the same per-clip guarantee without a host tensor."""
+    if gamma is not None:
+        def gamma_fn(i, shape):
+            return samplers.gamma_noise((hi - lo,) + tuple(shape[1:]), gamma[0], gamma[1], init_seed, clip0=lo,
+                                        step=samplers.GAMMA_INIT_STEP + i, device=dev)
+        return gamma_fn
+
     def init_fn(i, shape):
         outs = []
         for g in range(lo, hi):
@@ -279,8 +305,8 @@ def video_gen_sharded(config, scorenet, cond_all: torch.Tensor, rank: int, world
         cond = cond.to(dev)
         k = task_index(config, task)
         philox_seed, init_seed = task_seed(philox_seed, k), task_seed(init_seed, k)
-    local = video_gen_clips(config, scorenet, cond, init_fn=clip_init_fn(init_seed, lo, hi, dev), clip_offset=lo,
-                            philox_seed=philox_seed, **kw)
+    init_fn = clip_init_fn(init_seed, lo, hi, dev, gamma=gamma_init_params(config, scorenet))
+    local = video_gen_clips(config, scorenet, cond, init_fn=init_fn, clip_offset=lo, philox_seed=philox_seed, **kw)
     return gather_clips(local, n, rank, world)
 
 
@@ -353,7 +379,8 @@ def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
             kw["philox_seed"] = task_seed(kw["philox_seed"], k)
         if init_seed is not None:
             lo = kw.get("clip_offset", 0)
-            kw["init_fn"] = clip_init_fn(task_seed(init_seed, k), lo, lo + X.shape[0], dev)
+            kw["init_fn"] = clip_init_fn(task_seed(init_seed, k), lo, lo + X.shape[0], dev,
+                                         gamma=gamma_init_params(config, scorenet))
         frames = video_gen_clips(config, scorenet, cond.to(dev), nfp, **kw)
         metrics = None
         if real is not None and real.shape[1] < frames.shape[1]:

@@ -10,10 +10,17 @@ program and one fused update kernel (x0-prediction, clamp, posterior mean, + sig
 synchronised with the host unless ``log`` / ``verbose`` ask for the reference's diagnostics.
 Schedule coefficients are computed with the same fp32 torch expressions as the reference so they are
 bit-identical.
+
+Gamma noise (``gamma=True``, a model trained with ``model.gamma``): the per-step noise
+``(G - k_cum theta) / sqrt(1 - alpha)`` with ``G ~ Gamma(k_cum, scale theta)`` (models/__init__.py:319-322) is drawn
+inside the same fused update launch (``MCVD_F_GAMMA``), from a Philox stream keyed like the normal one; the
+reference draws it on the CPU and copies it to the GPU every step.  Without ``philox_seed`` the stream's seed is
+drawn from torch's default generator, so ``torch.manual_seed`` reproduces a run.
 """
 from __future__ import annotations
 
 import logging
+import math
 from typing import List, Optional
 
 import numpy as np
@@ -42,6 +49,53 @@ def _schedule(net, subsample_steps):
         alphas_prev = torch.cat([alphas[1:], torch.tensor([1.0])])
         betas = 1.0 - torch.div(alphas, alphas_prev)
     return steps, alphas, alphas_prev, betas
+
+
+# Philox step tags of the Gamma draws outside the per-step noise (which uses the step index i < L): the t_min
+# warm start of step i and, in the runner, x_T of AR block i
+GAMMA_WARM_STEP = 1 << 30
+GAMMA_INIT_STEP = 1 << 29
+
+
+def _gamma_schedule(net, subsample_steps):
+    """models/__init__.py:223-240: ``k_cum`` and ``theta_t``, index-selected with the subsampled steps."""
+    ks_cum, thetas = net.k_cum.detach().cpu(), net.theta_t.detach().cpu()
+    if subsample_steps is not None and subsample_steps < len(ks_cum):
+        skip = len(ks_cum) // subsample_steps
+        sel = torch.tensor(list(range(0, len(ks_cum), skip)))
+        ks_cum, thetas = ks_cum.index_select(0, sel), thetas.index_select(0, sel)
+    return ks_cum, thetas
+
+
+def _gamma_params(ks_cum, thetas, alphas, i):
+    """(shape, scale) of step i's centred Gamma draw: noise = (G - k theta) / sqrt(1 - alpha) = scale * (G' - k),
+    G' ~ Gamma(k, 1), with k = ks_cum[i] and scale = theta_i / sqrt(1 - alpha_i)."""
+    return float(ks_cum[i]), float(thetas[i]) / math.sqrt(float(1 - alphas[i]))
+
+
+def draw_seed() -> int:
+    """One 62-bit Philox seed from torch's default generator."""
+    return int(torch.randint(0, 1 << 62, (1,)).item())
+
+
+def gamma_noise(shape, k, theta, seed, clip0=0, step=0, scale=1.0, device=None) -> torch.Tensor:
+    """``scale * (G - k * theta)`` with ``G ~ Gamma(k, scale theta)`` per element of an NCHW tensor, drawn on the GPU by
+    ``MCVD_OP_NOISE`` from the Philox stream keyed by (seed, clip ``clip0 + b``, step tag ``step``, element)."""
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    if dev.type != "cuda":
+        raise RuntimeError("mcvd_b200.samplers.gamma_noise draws on CUDA devices only (no CPU fallback)")
+    B, C, H, W = shape
+    out = torch.empty(tuple(shape), device=dev, dtype=torch.float32)
+    if out.numel() == 0:
+        return out
+    op = lib.McvdOp()
+    op.kind, op.flags, op.B, op.H, op.W, op.C0 = lib.OP_NOISE, lib.F_GAMMA, B, H, W, C
+    op.i0, op.i1, op.i2, op.i3 = int(seed & 0x7FFFFFFF), int((seed >> 31) & 0x7FFFFFFF), int(clip0), int(step)
+    op.f5, op.f6, op.f7 = float(scale), float(k), float(theta)
+    op.dst = out.data_ptr()
+    with torch.cuda.device(dev):
+        lib.run_program(lib.make_ops([op]), 1, torch.cuda.current_stream(dev).cuda_stream)
+    return out
 
 
 class _Loop:
@@ -84,7 +138,8 @@ class _Loop:
         self.eng.run_step_graphed(self.P)
         self.launches += self.P.step_launches
 
-    def update(self, k0, k1, ca, cb, cc, sigma, clip, noise=None, philox=None, step=0):
+    def update(self, k0, k1, ca, cb, cc, sigma, clip, noise=None, philox=None, step=0, gamma=None):
+        """``gamma = (shape, scale)``: with ``philox``, z is the centred Gamma draw instead of the normal one."""
         u = self.u
         u.f0, u.f1, u.f2, u.f3, u.f4, u.f5 = float(k0), float(k1), float(ca), float(cb), float(cc), float(sigma)
         fl = lib.F_CLIP if clip else 0
@@ -93,6 +148,9 @@ class _Loop:
                 seed, clip0 = philox
                 fl |= lib.F_PHILOX
                 u.i0, u.i1, u.i2, u.i3 = int(seed & 0x7FFFFFFF), int((seed >> 31) & 0x7FFFFFFF), int(clip0), int(step)
+                if gamma is not None:
+                    fl |= lib.F_GAMMA
+                    u.f6, u.f7 = float(gamma[0]), float(gamma[1])
             else:
                 self.P.noise.copy_(noise.reshape(self.P.noise.shape))
         u.flags = fl
@@ -122,6 +180,18 @@ def _log_line(tag, i, L, grad, x, c_alpha, verbose, log):
         logging.info(msg)
 
 
+def _warm_start(lp, alpha, warm_noise, gamma, philox_seed, clip_offset, i):
+    """``t_min`` warm start (models/__init__.py:146-155, 272-279): x = sqrt(a) x + sqrt(1 - a) z.  z is
+    ``warm_noise`` if given, else the centred Gamma draw of step i (in the update launch) for a Gamma model, else
+    ``torch.randn``."""
+    if warm_noise is None and gamma is not None:
+        lp.update(0.0, 0.0, 0.0, alpha.sqrt().item(), 0.0, (1 - alpha).sqrt().item(), False,
+                  philox=(philox_seed, clip_offset), step=GAMMA_WARM_STEP + i, gamma=gamma)
+        return
+    z0 = warm_noise if warm_noise is not None else torch.randn(lp.P.noise.shape, device=lp.dev)
+    lp.update(0.0, 0.0, 0.0, alpha.sqrt().item(), 0.0, (1 - alpha).sqrt().item(), False, noise=z0)
+
+
 @torch.no_grad()
 def ddpm_sampler(x_mod, scorenet, cond=None, just_beta=False, final_only=False, denoise=True, subsample_steps=None,
                  same_noise=False, noise_val=None, frac_steps=None, verbose=False, log=False, clip_before=True,
@@ -132,17 +202,26 @@ def ddpm_sampler(x_mod, scorenet, cond=None, just_beta=False, final_only=False, 
     Extensions (keyword-only in practice): ``noise_list`` = per-step injected noise (L-1 tensors) for
     parity tests; ``philox_seed`` / ``clip_offset`` = draw the noise in-kernel from a counter-based
     stream keyed by the GLOBAL clip index, so a clip gets the same noise on any GPU.  With neither, the
-    noise is ``torch.randn_like`` as in the reference (:324).
+    noise is ``torch.randn_like`` as in the reference (:324).  ``warm_noise`` = injected ``z`` of the
+    ``t_min`` warm start.  With ``gamma`` the injected tensors are the reference's standardised noise
+    ``(G - k theta) / sqrt(1 - alpha)``; otherwise the Gamma draws are in-kernel (Philox seed drawn from torch's
+    default generator when ``philox_seed`` is None).
     """
-    if gamma:
-        raise NotImplementedError("gamma=True is not accelerated (reference models/__init__.py:214,319-322)")
     t_min = -1 if t_min is None else t_min
+    if gamma and philox_seed is None:
+        philox_seed = draw_seed()
     lp = _Loop(x_mod, scorenet, cond)
     try:
         steps, alphas, alphas_prev, betas = _schedule(lp.net, subsample_steps)
+        if gamma:
+            ks_cum, thetas = _gamma_schedule(lp.net, subsample_steps)             # :223-224, 238-240
         if frac_steps is not None:                                             # :249-256
             steps = steps[int((1 - frac_steps) * len(steps)):]
             alphas, alphas_prev, betas = alphas[steps], alphas_prev[steps], betas[steps]
+            if gamma:
+                ks_cum, thetas = ks_cum[steps], thetas[steps]
+        gp = (lambda j: _gamma_params(ks_cum, thetas, alphas, j)) if gamma else (lambda j: None)
+        tag = "DDPM gamma" if gamma else "DDPM"
         if same_noise and noise_val is None:                                    # :258-259
             noise_val = x_mod.detach().clone()
         L = len(steps)
@@ -152,8 +231,7 @@ def ddpm_sampler(x_mod, scorenet, cond=None, just_beta=False, final_only=False, 
             if step < t_min * len(alphas):                                      # :269-270 (init_prev_t warm start)
                 continue
             if not x_transf and t_min > 0:                                      # :272-279: noise x to this level
-                z0 = warm_noise if warm_noise is not None else torch.randn(lp.P.noise.shape, device=lp.dev)
-                lp.update(0.0, 0.0, 0.0, alphas[i].sqrt().item(), 0.0, (1 - alphas[i]).sqrt().item(), False, noise=z0)
+                _warm_start(lp, alphas[i], warm_noise, gp(i), philox_seed, clip_offset, i)
             x_transf = True
             c_beta, c_alpha, c_alpha_prev = betas[i], alphas[i], alphas_prev[i]
             lp.eps(float(step))                                                 # :283-284
@@ -178,15 +256,15 @@ def ddpm_sampler(x_mod, scorenet, cond=None, just_beta=False, final_only=False, 
                 if not final_only:
                     images.append(lp.state().to("cpu"))
                 if want_log:
-                    _log_line("DDPM", i, L, lp.eps_nchw(), lp.state(), c_alpha, verbose, log)
+                    _log_line(tag, i, L, lp.eps_nchw(), lp.state(), c_alpha, verbose, log)
                 if sigma != 0.0:  # x += sigma * z  == update with x0-coefficient 0 and x-coefficient 1
                     lp.update(0.0, 0.0, 0.0, 1.0, 0.0, sigma, False, noise=noise,
                               philox=None if philox_seed is None or noise is not None else (philox_seed, clip_offset),
-                              step=i)
+                              step=i, gamma=gp(i))
             else:
                 lp.update(k0.item(), k1.item(), ca.item(), cb.item(), 0.0, sigma, clip_before, noise=noise,
                           philox=None if philox_seed is None or noise is not None else (philox_seed, clip_offset),
-                          step=i)
+                          step=i, gamma=gp(i))
         if denoise:                                                             # :331-335
             lp.eps(float(L - 1))
             lp.update(0.0, 0.0, 0.0, 1.0, -(1 - alphas[-1]).sqrt().item(), 0.0, False)
@@ -202,14 +280,21 @@ def ddpm_sampler(x_mod, scorenet, cond=None, just_beta=False, final_only=False, 
 
 @torch.no_grad()
 def ddim_sampler(x_mod, scorenet, cond=None, final_only=False, denoise=True, subsample_steps=None, verbose=False,
-                 log=True, clip_before=True, t_min=-1, gamma=False, warm_noise: Optional[torch.Tensor] = None, **kwargs):
-    """Reference ``ddim_sampler`` (models/__init__.py:103-203): x = sqrt(a_prev) x0 + sqrt(1 - a_prev) eps."""
-    if gamma:
-        raise NotImplementedError("gamma=True is not accelerated")
+                 log=True, clip_before=True, t_min=-1, gamma=False, warm_noise: Optional[torch.Tensor] = None,
+                 philox_seed=None, clip_offset=0, **kwargs):
+    """Reference ``ddim_sampler`` (models/__init__.py:103-203): x = sqrt(a_prev) x0 + sqrt(1 - a_prev) eps.
+
+    Deterministic except for the ``t_min`` warm start; with ``gamma`` its noise is the in-kernel Gamma draw keyed by
+    ``philox_seed`` / ``clip_offset`` (seed drawn from torch's default generator when None), or ``warm_noise``."""
     t_min = -1 if t_min is None else t_min
+    if gamma and philox_seed is None:
+        philox_seed = draw_seed()
     lp = _Loop(x_mod, scorenet, cond)
     try:
         steps, alphas, alphas_prev, betas = _schedule(lp.net, subsample_steps)
+        if gamma:
+            ks_cum, thetas = _gamma_schedule(lp.net, subsample_steps)                  # :118-119, 134-136
+        gp = (lambda j: _gamma_params(ks_cum, thetas, alphas, j)) if gamma else (lambda j: None)
         L = len(steps)
         images = []
         x_transf = False
@@ -217,8 +302,7 @@ def ddim_sampler(x_mod, scorenet, cond=None, final_only=False, denoise=True, sub
             if step < t_min * len(alphas):                                           # :143-144
                 continue
             if not x_transf and t_min > 0:                                           # :146-153
-                z0 = warm_noise if warm_noise is not None else torch.randn(lp.P.noise.shape, device=lp.dev)
-                lp.update(0.0, 0.0, 0.0, alphas[i].sqrt().item(), 0.0, (1 - alphas[i]).sqrt().item(), False, noise=z0)
+                _warm_start(lp, alphas[i], warm_noise, gp(i), philox_seed, clip_offset, i)
             x_transf = True
             c_alpha, c_alpha_prev = alphas[i], alphas_prev[i]
             lp.eps(float(step))
@@ -227,7 +311,7 @@ def ddim_sampler(x_mod, scorenet, cond=None, final_only=False, denoise=True, sub
             if not final_only:
                 images.append(lp.state().to("cpu"))
             if (verbose or log) and (i == 0 or (i + 1) % max(L // 10, 1) == 0):
-                _log_line("DDIM", i, L, lp.eps_nchw(), lp.state(), c_alpha, verbose, log)
+                _log_line("DDIM gamma" if gamma else "DDIM", i, L, lp.eps_nchw(), lp.state(), c_alpha, verbose, log)
         if denoise:                                                                 # :194-196
             lp.eps(float(L - 1))
             lp.update(0.0, 0.0, 0.0, 1.0, -(1 - alphas[-1]).sqrt().item(), 0.0, False)
@@ -244,6 +328,7 @@ def ddim_sampler(x_mod, scorenet, cond=None, final_only=False, denoise=True, sub
 def FPNDM_sampler(x_mod, scorenet, cond=None, final_only=False, denoise=True, subsample_steps=None, verbose=False,
                   log=True, clip_before=True, t_min=-1, gamma=False, **kwargs):
     """Reference ``FPNDM_sampler`` + ``pndm.gen_order_4`` (models/__init__.py:39-99, models/pndm.py:3-52).
+    Deterministic; ``gamma`` is accepted and ignored, as in the reference.
 
     Replicated as written: alphas looked up through the flipped copy with the +1 offset, steps_next =
     [-1] + steps[:-1], fractional mid-timesteps fed to the network, no final denoise call.  Every
