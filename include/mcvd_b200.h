@@ -152,6 +152,26 @@ enum {
    * centred Gamma draw f7 * (G - f6).  x_T of a Gamma-noise model (runners/ncsn_runner.py:1471-1474, 1546-1549)
    * without a host tensor.  src0 is not read. */
   MCVD_OP_NOISE = 18,
+  /* LPIPS input of generated and real frames (runners/ncsn_runner.py:1427-1430, 1590-1591, 1606-1607:
+   * ToPILImage -> convert("RGB") -> Resize((128, 128)) -> ToTensor -> Normalize(0.5, 0.5), then ScalingLayer,
+   * models/networks_basic.py:89-96).  src0 = pred, src1 = real, both [B, C0*i0, i1, i1] fp32 (i0 frames of C0 = 1|3
+   * channels, side i1), clamped to [0, 1]; u8 = trunc(x * 255); PIL's two-pass 8-bit bilinear resize with the
+   * coefficient table w = int32 [128][2 + i2] (per output row/column: first source index, taps used, i2 22-bit
+   * coefficients; mcvd_b200/lpips.py computes it); dst = fp32 NHWC [2*B*i0, 128, 128, 4] (pred frames, then real
+   * frames; channel 3 is zero).  H = W = 128. */
+  MCVD_OP_LPIPS_PREP = 19,
+  /* NHWC direct convolution + bias + ReLU on the CUDA cores (fp32 FFMA implicit GEMM): one layer of torchvision's
+   * alexnet().features (models/pretrained_networks.py:56-94).  src0 [B, i3, i4, C0] (C0 a multiple of 4);
+   * MCVD_F_POOL: the conv reads the 3x3 / stride-2 max-pool of src0 instead (features[2], [5]);
+   * i0 = kernel size, i1 = stride, i2 = padding; w = fp32 [i0][i0][C0][Cout] (K-major), bias [Cout], Cout a multiple
+   * of 64; dst [B, H, W, Cout] with H, W = (input side + 2 i2 - i0) / i1 + 1. */
+  MCVD_OP_CONV_RELU = 20,
+  /* LPIPS head of one AlexNet tap (models/networks_basic.py:73-84, eval_models.py:35-37): per position
+   * f / (sqrt(sum_c f^2) + 1e-10) of both maps, the squared difference weighted by lin_k (w = fp32 [C0]) summed over
+   * channels, mean over the H*W positions.  src0 = pred features, src1 = real features, both [B, H, W, C0];
+   * dst = fp64 [B] per frame pair: i0 == 0 overwrites, i0 != 0 adds (the five taps summed in order).  Fixed
+   * reduction order, no atomics. */
+  MCVD_OP_LPIPS_LAYER = 21,
   MCVD_OP__COUNT
 };
 
@@ -165,6 +185,7 @@ enum {
 #define MCVD_F_PHILOX   (1 << 6)   /* DIFFUSION_UPDATE: draw z in-kernel                           */
 #define MCVD_F_ROUND    (1 << 7)   /* FRAME_METRICS: round the images before the grey conversion   */
 #define MCVD_F_GAMMA    (1 << 8)   /* DIFFUSION_UPDATE (with PHILOX), NOISE: centred Gamma(f6) * f7 */
+#define MCVD_F_POOL     (1 << 9)   /* CONV_RELU: 3x3 / stride-2 max-pool on the input read           */
 
 typedef struct McvdOp {
   int32_t kind;

@@ -35,6 +35,9 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_ATTENTION_UMMA: return launch_attention_umma(op, s);
     case MCVD_OP_FRAME_METRICS: return launch_frame_metrics(op, s);
     case MCVD_OP_NOISE: return launch_noise(op, s);
+    case MCVD_OP_LPIPS_PREP: return launch_lpips_prep(op, s);
+    case MCVD_OP_CONV_RELU: return launch_conv_relu(op, s);
+    case MCVD_OP_LPIPS_LAYER: return launch_lpips_layer(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -106,6 +109,40 @@ static int validate_one(const McvdOp& op, int idx) {
           set_error("op %d (kind %d): %s", idx, op.kind, why);
           return -1;
         }
+      }
+      break;
+    case MCVD_OP_LPIPS_PREP:
+      if (!op.src1 || !op.w) {
+        set_error("op %d LPIPS_PREP: null real frames or resize table", idx);
+        return -1;
+      }
+      if (op.C0 != 1 && op.C0 != 3) {
+        set_error("op %d LPIPS_PREP: %d channels per frame (1 or 3)", idx, op.C0);
+        return -1;
+      }
+      if (op.H != 128 || op.W != 128) {
+        set_error("op %d LPIPS_PREP: output side %dx%d (must be 128x128)", idx, op.H, op.W);
+        return -1;
+      }
+      if (op.i0 < 1 || op.i1 < 1 || op.i2 < 1 || 2LL * op.B * op.i0 > 65535) {
+        set_error("op %d LPIPS_PREP: %d frames of side %d, %d taps, batch %d", idx, op.i0, op.i1, op.i2, op.B);
+        return -1;
+      }
+      break;
+    case MCVD_OP_CONV_RELU:
+      if (const char* why = conv_relu_error(op)) {
+        set_error("op %d CONV_RELU: %s", idx, why);
+        return -1;
+      }
+      if (misaligned(op.bias)) {
+        set_error("op %d CONV_RELU: bias must be 16-byte aligned", idx);
+        return -1;
+      }
+      break;
+    case MCVD_OP_LPIPS_LAYER:
+      if (!op.src1 || !op.w || op.C0 < 1) {
+        set_error("op %d LPIPS_LAYER: null real features or lin weights, or %d channels", idx, op.C0);
+        return -1;
       }
       break;
     default: break;

@@ -51,6 +51,12 @@ int launch_copy(const McvdOp& op, cudaStream_t s);
 int launch_attention_umma(const McvdOp& op, cudaStream_t s);
 int launch_frame_metrics(const McvdOp& op, cudaStream_t s);
 int launch_noise(const McvdOp& op, cudaStream_t s);
+int launch_lpips_prep(const McvdOp& op, cudaStream_t s);
+int launch_conv_relu(const McvdOp& op, cudaStream_t s);
+int launch_lpips_layer(const McvdOp& op, cudaStream_t s);
+
+// NULL, or why the geometry of a MCVD_OP_CONV_RELU op is unusable
+const char* conv_relu_error(const McvdOp& op);
 
 // NULL, or why the Gamma parameters (f6 = shape, f7 = scale) of an op with MCVD_F_GAMMA are unusable
 const char* gamma_params_error(const McvdOp& op);

@@ -30,6 +30,9 @@ OP_ATTENTION_UMMA = 15
 OP_CONV_UMMA2 = 16
 OP_FRAME_METRICS = 17
 OP_NOISE = 18
+OP_LPIPS_PREP = 19
+OP_CONV_RELU = 20
+OP_LPIPS_LAYER = 21
 
 F_ACT_IN = 1 << 0
 F_ACT_OUT = 1 << 1
@@ -40,6 +43,7 @@ F_CLIP = 1 << 5
 F_PHILOX = 1 << 6
 F_ROUND = 1 << 7
 F_GAMMA = 1 << 8
+F_POOL = 1 << 9
 
 ABI_VERSION = 5
 

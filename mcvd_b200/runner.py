@@ -352,7 +352,7 @@ def best_of_repeats(per_frame: torch.Tensor, preds_per_test: int):
 @torch.no_grad()
 def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[int] = None,
                    tasks: Optional[List[str]] = None, num_frames_pred: Optional[int] = None,
-                   **gen_kw) -> Dict[str, Tuple[torch.Tensor, Optional[dict]]]:
+                   lpips: Optional[Callable] = None, **gen_kw) -> Dict[str, Tuple[torch.Tensor, Optional[dict]]]:
     """One test batch of the reference's ``video_gen`` (runners/ncsn_runner.py:1392-1395, 1444-1915), every task.
 
     ``X`` is [B, T, C, S, S] in [0, 1].  Every test clip is repeated ``preds_per_test`` times (``repeat_interleave``,
@@ -361,6 +361,8 @@ def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
     ``num_frames``).  Returns ``{task: (frames [B*p, C*nfp, S, S] in [0, 1], metrics)}``.  ``metrics`` holds
     per-clip ``mse`` / ``psnr`` / ``ssim`` of the best repeat and the ``per_frame`` values, or is ``None`` for
     ``gen``, which has no ground truth, and for a task that predicts past the real frames of ``X`` (:1573-1579).
+    With an ``lpips`` (a ``mcvd_b200.lpips.LPIPS``), ``metrics`` also holds ``per_frame_lpips`` [B*p, nfp] and per-clip
+    ``lpips``: the mean over frames of the best (lowest) repeat (:1606-1609, 2199).
 
     ``gen_kw`` go to ``video_gen_clips``.  A ``philox_seed`` among them is replaced by the task's
     (``task_seed``).  An ``init_seed`` draws x_T per global clip (``clip_init_fn``, clips numbered from
@@ -390,16 +392,21 @@ def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
             per_frame = frame_metrics(config, frames, real.to(dev))
             mse, psnr, ssim = best_of_repeats(per_frame, p)
             metrics = {"mse": mse, "psnr": psnr, "ssim": ssim, "per_frame": per_frame}
+            if lpips is not None:
+                per_frame_lpips = lpips(frames, real.to(dev), config.data.channels)
+                metrics["lpips"] = per_frame_lpips.mean(1).reshape(-1, p).min(-1).values
+                metrics["per_frame_lpips"] = per_frame_lpips
         out[task] = (frames, metrics)
     return out
 
 
 @torch.no_grad()
 def evaluate_clips(config, scorenet, X: torch.Tensor, preds_per_test: Optional[int] = None,
-                   num_frames_pred: Optional[int] = None, **gen_kw):
+                   num_frames_pred: Optional[int] = None, lpips: Optional[Callable] = None, **gen_kw):
     """Task (1) of ``evaluate_tasks``: prediction, or interpolation for a model with future frames, with no
     conditioning masked (runners/ncsn_runner.py:1458-1459).  ``X`` is [B, T, C, S, S] in [0, 1].  Returns
-    (frames [B*p, C*nfp, S, S] in [0, 1], dict of per-clip mse / psnr / ssim tensors and ``per_frame``)."""
+    (frames [B*p, C*nfp, S, S] in [0, 1], dict of per-clip mse / psnr / ssim tensors and ``per_frame``, plus
+    ``lpips`` and ``per_frame_lpips`` with an ``lpips``)."""
     task = "interp" if getattr(config.data, "num_frames_future", 0) > 0 else "pred"
     return evaluate_tasks(config, scorenet, X, preds_per_test, tasks=[task], num_frames_pred=num_frames_pred,
-                          **gen_kw)[task]
+                          lpips=lpips, **gen_kw)[task]
