@@ -172,6 +172,29 @@ enum {
    * dst = fp64 [B] per frame pair: i0 == 0 overwrites, i0 != 0 adds (the five taps summed in order).  Fixed
    * reduction order, no atomics. */
   MCVD_OP_LPIPS_LAYER = 21,
+  /* I3D input of videos for FVD (models/fvd/fvd.py:160-186 preprocess_single, runners/ncsn_runner.py:1918-1923
+   * to_i3d): src0 = frames [B, C0*i0, i1, i1] fp32 (i0 frames of C0 = 1|3 channels, side i1, frame-major), bilinear
+   * resize to i2 x i3 (F.interpolate align_corners=False: src = (dst + 0.5) * i1 / size - 0.5, clamped at 0), centre
+   * crop to 224x224 at ((i2 - 224) / 2, (i3 - 224) / 2), (x - 0.5) * 2, no clamp; a grey frame is replicated to RGB.
+   * dst = fp32 NDHWC [B, i0, 224, 224, 4], channel 3 zero.  H = W = 224; B * i0 <= 65535. */
+  MCVD_OP_I3D_PREP = 22,
+  /* NDHWC 3-D convolution + bias + ReLU (fp32 FFMA implicit GEMM): one Unit3D of InceptionI3d with its BatchNorm3d
+   * folded into w and bias on the host (models/fvd/pytorch_i3d.py:37-103).  src0 [B, i4, i5, i5, C0] (C0 a multiple
+   * of 4); kernel i0 x i1 x i1, stride i2 x i3 x i3; TF-SAME padding from the input size (compute_pad, :71-96):
+   * per axis pad = max(k - (in % s ? in % s : s), 0), front pad / 2; output [B, To, H, W] with
+   * To = (i4 + pad_t - i0) / i2 + 1 and H = W = (i5 + pad_s - i1) / i3 + 1 (= ceil(in / stride)).
+   * w = fp32 [i0][i1][i1][C0][Cout] (K-major), bias [Cout], Cout a multiple of 8.  The output is channels
+   * [i7, i7 + Cout) of dst [B, To, H, W, i6] (i6 = channel pitch >= i7 + Cout, both multiples of 4); other channels
+   * are not written, so the four branches of an Inception block write their concat in place (:127-132). */
+  MCVD_OP_CONV3D = 23,
+  /* MaxPool3dSamePadding (models/fvd/pytorch_i3d.py:7-34): zero padding as CONV3D's (zeros take part in the max),
+   * window i0 x i1 x i1, stride i2 x i3 x i3; src0 [B, i4, i5, i5, C0] (C0 a multiple of 4), dst [B, To, H, W, C0]
+   * with To, H, W as for CONV3D. */
+  MCVD_OP_MAXPOOL3D = 24,
+  /* InceptionI3d head (models/fvd/pytorch_i3d.py:275-315): AvgPool3d([2, 7, 7], stride 1), the 1x1x1 logits conv
+   * with bias (w = fp32 [C0][Cout], bias fp32 [Cout]), mean over time.  src0 [B, i4, 7, 7, C0] (i5 = 7, i4 >= 2),
+   * dst fp64 [B, Cout] (Cout <= 512, C0 <= 6144); all in fp64, fixed reduction order, no atomics.  H = W = 1. */
+  MCVD_OP_I3D_HEAD = 25,
   MCVD_OP__COUNT
 };
 

@@ -38,6 +38,10 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_LPIPS_PREP: return launch_lpips_prep(op, s);
     case MCVD_OP_CONV_RELU: return launch_conv_relu(op, s);
     case MCVD_OP_LPIPS_LAYER: return launch_lpips_layer(op, s);
+    case MCVD_OP_I3D_PREP: return launch_i3d_prep(op, s);
+    case MCVD_OP_CONV3D: return launch_conv3d(op, s);
+    case MCVD_OP_MAXPOOL3D: return launch_maxpool3d(op, s);
+    case MCVD_OP_I3D_HEAD: return launch_i3d_head(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -145,6 +149,25 @@ static int validate_one(const McvdOp& op, int idx) {
         return -1;
       }
       break;
+    case MCVD_OP_I3D_PREP:
+    case MCVD_OP_CONV3D:
+    case MCVD_OP_MAXPOOL3D:
+    case MCVD_OP_I3D_HEAD: {
+      const char* why = op.kind == MCVD_OP_I3D_PREP ? i3d_prep_error(op)
+                        : op.kind == MCVD_OP_CONV3D  ? conv3d_error(op)
+                        : op.kind == MCVD_OP_MAXPOOL3D ? maxpool3d_error(op)
+                                                       : i3d_head_error(op);
+      static const char* const names[] = {"I3D_PREP", "CONV3D", "MAXPOOL3D", "I3D_HEAD"};
+      if (why) {
+        set_error("op %d %s: %s", idx, names[op.kind - MCVD_OP_I3D_PREP], why);
+        return -1;
+      }
+      if (misaligned(op.bias)) {
+        set_error("op %d %s: bias must be 16-byte aligned", idx, names[op.kind - MCVD_OP_I3D_PREP]);
+        return -1;
+      }
+      break;
+    }
     default: break;
   }
   return 0;

@@ -54,9 +54,19 @@ int launch_noise(const McvdOp& op, cudaStream_t s);
 int launch_lpips_prep(const McvdOp& op, cudaStream_t s);
 int launch_conv_relu(const McvdOp& op, cudaStream_t s);
 int launch_lpips_layer(const McvdOp& op, cudaStream_t s);
+int launch_i3d_prep(const McvdOp& op, cudaStream_t s);
+int launch_conv3d(const McvdOp& op, cudaStream_t s);
+int launch_maxpool3d(const McvdOp& op, cudaStream_t s);
+int launch_i3d_head(const McvdOp& op, cudaStream_t s);
 
 // NULL, or why the geometry of a MCVD_OP_CONV_RELU op is unusable
 const char* conv_relu_error(const McvdOp& op);
+
+// NULL, or why an op of the I3D kinds is unusable (shared by validation and launch; i3d.cu)
+const char* i3d_prep_error(const McvdOp& op);
+const char* conv3d_error(const McvdOp& op);
+const char* maxpool3d_error(const McvdOp& op);
+const char* i3d_head_error(const McvdOp& op);
 
 // NULL, or why the Gamma parameters (f6 = shape, f7 = scale) of an op with MCVD_F_GAMMA are unusable
 const char* gamma_params_error(const McvdOp& op);

@@ -33,6 +33,10 @@ OP_NOISE = 18
 OP_LPIPS_PREP = 19
 OP_CONV_RELU = 20
 OP_LPIPS_LAYER = 21
+OP_I3D_PREP = 22
+OP_CONV3D = 23
+OP_MAXPOOL3D = 24
+OP_I3D_HEAD = 25
 
 F_ACT_IN = 1 << 0
 F_ACT_OUT = 1 << 1

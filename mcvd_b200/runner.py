@@ -3,7 +3,9 @@
 Restates (does not copy) ``runners/ncsn_runner.py``: ``conditioning_fn`` (:104-147), the AR loop of
 ``NCSNRunner.video_gen`` (:1501-1570), its three tasks -- prediction or interpolation, prediction with a
 future-frame model, unconditional generation -- chosen by the mode table of ``get_mode`` (:208-227), and
-``get_sampler`` (:2702-2714); the dataset, LPIPS / FVD, gif and checkpoint-sweep code around them is out of scope.
+``get_sampler`` (:2702-2714); the dataset, gif and checkpoint-sweep code around them is out of scope.  The
+per-clip metrics (MSE, PSNR, SSIM, and LPIPS with ``mcvd_b200.lpips``) and FVD's I3D features (with
+``mcvd_b200.fvd``) of each task are computed on the GPU by ``evaluate_tasks``.
 
 Multi-GPU: the reference wraps the network in ``torch.nn.DataParallel`` (:1377) and re-broadcasts all
 weights on every one of the 101 x n_iter network calls.  Here every clip (batch element) is
@@ -352,7 +354,8 @@ def best_of_repeats(per_frame: torch.Tensor, preds_per_test: int):
 @torch.no_grad()
 def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[int] = None,
                    tasks: Optional[List[str]] = None, num_frames_pred: Optional[int] = None,
-                   lpips: Optional[Callable] = None, **gen_kw) -> Dict[str, Tuple[torch.Tensor, Optional[dict]]]:
+                   lpips: Optional[Callable] = None, i3d: Optional[Callable] = None,
+                   **gen_kw) -> Dict[str, Tuple[torch.Tensor, Optional[dict]]]:
     """One test batch of the reference's ``video_gen`` (runners/ncsn_runner.py:1392-1395, 1444-1915), every task.
 
     ``X`` is [B, T, C, S, S] in [0, 1].  Every test clip is repeated ``preds_per_test`` times (``repeat_interleave``,
@@ -364,6 +367,14 @@ def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
     With an ``lpips`` (a ``mcvd_b200.lpips.LPIPS``), ``metrics`` also holds ``per_frame_lpips`` [B*p, nfp] and per-clip
     ``lpips``: the mean over frames of the best (lowest) repeat (:1606-1609, 2199).
 
+    With an ``i3d`` (a ``mcvd_b200.fvd.I3D``), every task whose video has at least 10 frames (``fvd_videos``: the
+    reference's gate, :1311-1332) and whose real frames cover the prediction also gets ``i3d_fake`` [B*p, 400] and
+    ``i3d_real`` [B, 400] float64 features and the ``fvd_summary`` keys ``fvd``, ``fvd_traj_mean``, ``fvd_traj_std``
+    and ``fvd_traj_conf95`` of this batch (:1918-1982, 2217-2229).  ``gen`` then gets a dict of only those keys,
+    scored against the real videos of task (2) when the model runs it and of task (1) otherwise (:1975-1977).  The
+    reference computes FVD over its whole test set: concatenate the features of every batch and call
+    ``fvd.fvd_summary`` once.
+
     ``gen_kw`` go to ``video_gen_clips``.  A ``philox_seed`` among them is replaced by the task's
     (``task_seed``).  An ``init_seed`` draws x_T per global clip (``clip_init_fn``, clips numbered from
     ``clip_offset``) from the task's seed.  ``init_fn`` and ``noise_fn`` reach every task unchanged.
@@ -373,6 +384,7 @@ def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
     dev = next(scorenet.parameters()).device
     init_seed = gen_kw.pop("init_seed", None)
     out = {}
+    C = config.data.channels
     for task in (tasks_for(config) if tasks is None else tasks):
         real, cond, nfp = task_inputs(config, X, task, None if task == "interp" else num_frames_pred)
         k = task_index(config, task)
@@ -396,17 +408,59 @@ def evaluate_tasks(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
                 per_frame_lpips = lpips(frames, real.to(dev), config.data.channels)
                 metrics["lpips"] = per_frame_lpips.mean(1).reshape(-1, p).min(-1).values
                 metrics["per_frame_lpips"] = per_frame_lpips
+            if i3d is not None:
+                fake_v, real_v = fvd_videos(config, task, cond, frames, real)
+                if fake_v.shape[1] // C >= FVD_MIN_FRAMES:
+                    metrics.update(_fvd_metrics(i3d, fake_v, real_v[::p], C, p))
+        if task == "gen" and i3d is not None and frames.shape[1] // C >= FVD_MIN_FRAMES:
+            future = getattr(config.data, "num_frames_future", 0) > 0
+            src = "pred" if future and "pred" in tasks_for(config) else ("interp" if future else "pred")
+            real_s, cond_s, nfp_s = task_inputs(config, X, src, None if src == "interp" else num_frames_pred)
+            if real_s.shape[1] < C * nfp_s:
+                logging.warning("evaluate_tasks: X is too short for the real videos of task %r; no FVD for 'gen'", src)
+            else:
+                _, real_v = fvd_videos(config, src, cond_s, real_s, real_s)
+                if real_v.shape[1] // C < MIN_I3D_FRAMES:
+                    logging.warning("evaluate_tasks: the real videos of task %r have %d frames, too few for I3D; no "
+                                    "FVD for 'gen'", src, real_v.shape[1] // C)
+                else:
+                    metrics = _fvd_metrics(i3d, frames, real_v[::p], C, p)
         out[task] = (frames, metrics)
     return out
 
 
+FVD_MIN_FRAMES = 10          # video_gen scores a task's FVD only when its videos have at least 10 frames
+MIN_I3D_FRAMES = 9           # InceptionI3d's shortest input
+
+
+def fvd_videos(config, task: str, cond: torch.Tensor, frames: torch.Tensor, real: torch.Tensor):
+    """(fake, real) videos [N, C*L, S, S] in [0, 1] the reference scores with I3D for ``task``
+    (runners/ncsn_runner.py:1925-1972): the past conditioning frames, then the generated (or real) frames, then for
+    interpolation the future frames.  ``cond`` is the task's conditioning in the model's range (``task_inputs``);
+    for ``gen`` the fake video is ``frames`` alone (:1980)."""
+    if task == "gen":
+        return frames, None
+    C, Fc = config.data.channels, config.data.num_frames_cond
+    c01 = inverse_data_transform(config, cond).to(frames.device)
+    past, future = c01[:, :C * Fc], (c01[:, C * Fc:] if task == "interp" else c01[:, :0])
+    return (torch.cat([past, frames, future], dim=1),
+            torch.cat([past, real.to(frames.device), future], dim=1))
+
+
+def _fvd_metrics(i3d, fake: torch.Tensor, real: torch.Tensor, channels: int, p: int) -> dict:
+    from .fvd import fvd_summary
+    f, r = i3d(fake, channels), i3d(real, channels)
+    return dict(i3d_fake=f, i3d_real=r, **fvd_summary(f, r, p))
+
+
 @torch.no_grad()
 def evaluate_clips(config, scorenet, X: torch.Tensor, preds_per_test: Optional[int] = None,
-                   num_frames_pred: Optional[int] = None, lpips: Optional[Callable] = None, **gen_kw):
+                   num_frames_pred: Optional[int] = None, lpips: Optional[Callable] = None,
+                   i3d: Optional[Callable] = None, **gen_kw):
     """Task (1) of ``evaluate_tasks``: prediction, or interpolation for a model with future frames, with no
     conditioning masked (runners/ncsn_runner.py:1458-1459).  ``X`` is [B, T, C, S, S] in [0, 1].  Returns
     (frames [B*p, C*nfp, S, S] in [0, 1], dict of per-clip mse / psnr / ssim tensors and ``per_frame``, plus
-    ``lpips`` and ``per_frame_lpips`` with an ``lpips``)."""
+    ``lpips`` and ``per_frame_lpips`` with an ``lpips``, and the FVD keys with an ``i3d``)."""
     task = "interp" if getattr(config.data, "num_frames_future", 0) > 0 else "pred"
     return evaluate_tasks(config, scorenet, X, preds_per_test, tasks=[task], num_frames_pred=num_frames_pred,
-                          lpips=lpips, **gen_kw)[task]
+                          lpips=lpips, i3d=i3d, **gen_kw)[task]
