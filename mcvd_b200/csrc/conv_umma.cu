@@ -23,13 +23,25 @@
 // Outputs at padding positions are computed and discarded (2..20 % of the rows).
 //
 // Warp roles (384 threads, one CTA per SM, persistent over 128-position x NT tiles):
-//   warps 0-2   producers: fp32 NHWC global -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2 stages)
-//               (generic-proxy stores + fence.proxy.async)
+//   warps 0-2   producers: raw fp32 NHWC stage in smem -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2 stages)
+//               (generic-proxy stores + fence.proxy.async).  Thread 0 also issues the TMA (cp.async.bulk.tensor)
+//               loads of the raw input boxes and norm-table rows, one K-block ahead of the conversion.
 //   warp  3     weight loader: cp.async.bulk (TMA 1-D) of pre-packed fp16 hi/lo smem images (ring of NB stages)
 //   warps 4-11  two consumer warpgroups, 64 rows of the tile each: wgmma m64nNTk16 from the slab and weight
 //               stages, then the epilogue straight from the accumulator registers (bias / residual / scale /
 //               SiLU, optional GroupNorm statistics of the stored output)
+//
+// Raw input stages.  The real pixels among consecutive padded-flat positions are consecutive NHWC pixels, so the
+// raw input of a slab is one run of rows of a 2-D {C_src, B*H*W} tensor map: one TMA box of HP rows (two when
+// HP > 256, the box-size limit), zero-filled past the end of the batch.  One-tap K-blocks (1x1 convs, the fused
+// shortcut segment) load and convert only the 128 rows of the tile's own positions.  The boxes are 64- / 128-byte
+// swizzled (KB = 16 / 32 channels per row) so that eight producers reading the same 16 bytes of eight consecutive
+// rows hit distinct banks.
+#include <cuda.h>
 #include <cuda_fp16.h>
+
+#include <algorithm>
+#include <cstring>
 
 #include "mcvd_common.cuh"
 #include "umma_ptx.cuh"
@@ -49,7 +61,15 @@ constexpr int NTHREADS = 384;   // 168 registers per thread: room for the 128 ac
 constexpr float STAT_SCALE = 65536.0f;   // fixed-point scale of the epilogue statistics
 constexpr int TAB_NB = 8;       // images whose norm-table rows are staged in smem per K-block
 constexpr int HP_MAX = 512;
-constexpr int MAX_RESIDENT = 12;   // K-blocks an input-stationary work item keeps resident (12 x 8 KB at KB = 32)
+constexpr int PPT = (HP_MAX + NPROD - 1) / NPROD;   // slab positions per producer thread
+constexpr int RAW_STAGES = 2;   // raw input stages: the loads of K-block g + 1 fly while K-block g is converted
+constexpr int MAX_RESIDENT = 12;   // K-blocks an input-stationary work item keeps resident (12 x 16 KB at KB = 32)
+
+// tiled tensor maps of the raw sources s0..s3 ({C_src, B*H*W}) and of the norm table; unused entries are zero
+struct ConvMaps {
+  CUtensorMap src[4];
+  CUtensorMap tab;
+};
 
 struct ConvArgs {
   const float* s0;
@@ -68,9 +88,12 @@ struct ConvArgs {
   int B, H, W, C0, C1, Cout;
   int ks;                // 1 or 3
   int Wp, Pimg;          // padded row pitch, positions per image
-  long long Qtot;        // total flat positions
+  int Qtot;              // total flat positions
   int KB;                // channels per K-block (16|32)
   int HP;                // halo slab positions (multiple of 8)
+  int boxn, nbox;        // rows per TMA box of the first segment's sources, boxes per K-block
+  int raw_off, raw_stage, tab_off;   // smem offset and size of a raw stage; its norm-table rows follow the pixels
+  int RA;                // raw stages: RAW_STAGES, or 1 where two do not fit (the loads then wait for the conversion)
   int halo0;             // slab index of the tile's first output position
   int nKB;               // K-blocks
   int NB;                // weight ring stages
@@ -84,10 +107,10 @@ struct ConvArgs {
 };
 
 // position decode: flat q -> pixel index (b*H + y)*W + x, or -1 for padding / out of range
-__device__ __forceinline__ int decode_pos(const ConvArgs& a, long long q, int& b_out) {
+__device__ __forceinline__ int decode_pos(const ConvArgs& a, int q, int& b_out) {
   if (q < 0 || q >= a.Qtot) return -1;
-  const int b = (int)(q / a.Pimg);
-  const int r = (int)(q - (long long)b * a.Pimg);
+  const int b = q / a.Pimg;
+  const int r = q - b * a.Pimg;
   const int rr = r / a.Wp, cc = r - rr * a.Wp;
   b_out = b;
   if (a.ks == 3) {
@@ -97,8 +120,20 @@ __device__ __forceinline__ int decode_pos(const ConvArgs& a, long long q, int& b
   return (b * a.H + rr) * a.W + cc;
 }
 
+// first pixel index at or after flat position q (B*H*W past the end): the first row of a raw TMA box
+__device__ __forceinline__ int first_raw(const ConvArgs& a, int q) {
+  q = max(q, 0);
+  if (q >= a.Qtot) return a.B * a.H * a.W;
+  if (a.ks == 1) return q;
+  const int b = q / a.Pimg;
+  const int r = q - b * a.Pimg;
+  const int rr = r / a.Wp, cc = r - rr * a.Wp;
+  if (rr == 0) return b * a.H * a.W;
+  return (b * a.H + (rr - 1)) * a.W + (cc == 0 ? 0 : cc - 1);
+}
+
 template <int NT>
-__global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
+__global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a, const __grid_constant__ ConvMaps maps) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int chunks = a.KB / 8;
   const uint32_t a_half_bytes = (uint32_t)chunks * a.HP * 16;       // one of hi / lo
@@ -107,15 +142,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
   const uint32_t b_stage_bytes = (uint32_t)(a.KB / 16) * b_step_bytes;
   uint8_t* a_base = smem_raw;
   uint8_t* b_base = a_base + (size_t)a.SA * a_stage_bytes;
-  float* tab_s = reinterpret_cast<float*>(b_base + (size_t)a.NB * b_stage_bytes);         // [2][TAB_NB][96]
-  unsigned long long* stat_s = reinterpret_cast<unsigned long long*>(tab_s + 2 * TAB_NB * 96);   // [NJ][2][NT]
+  uint8_t* raw_base = smem_raw + a.raw_off;                          // [RA][raw_stage], 1024-byte aligned
+  int* pinfo = reinterpret_cast<int*>(raw_base + (size_t)a.RA * a.raw_stage);   // [PPT][NPROD]
+  unsigned long long* stat_s = reinterpret_cast<unsigned long long*>(pinfo + PPT * NPROD);   // [NJ][2][NT]
   uint64_t* bars = reinterpret_cast<uint64_t*>(stat_s + (a.stats ? a.NJ * 2 * NT : 0));
-  // bars: a_full[SA], a_empty[SA], b_full[NB], b_empty[NB]
+  // bars: a_full[SA], a_empty[SA], b_full[NB], b_empty[NB], r_full[RA]
   const uint32_t bar0 = smem_u32(bars);
   auto A_FULL = [&](int i) { return bar0 + 8u * i; };
   auto A_EMPTY = [&](int i) { return bar0 + 8u * (a.SA + i); };
   auto B_FULL = [&](int i) { return bar0 + 8u * (2 * a.SA + i); };
   auto B_EMPTY = [&](int i) { return bar0 + 8u * (2 * a.SA + a.NB + i); };
+  auto R_FULL = [&](int i) { return bar0 + 8u * (2 * a.SA + 2 * a.NB + i); };
   const int groups_n = a.tiles_n / a.NPI;                 // work item t: m tile t / groups_n, n tiles of group t % groups_n
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -125,6 +162,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
     // consumers release a stage with one arrival per consumer warp (8)
     for (int i = 0; i < a.SA; ++i) { mbar_init(A_FULL(i), NPROD); mbar_init(A_EMPTY(i), 8); }
     for (int i = 0; i < a.NB; ++i) { mbar_init(B_FULL(i), 1); mbar_init(B_EMPTY(i), 8); }
+    for (int i = 0; i < a.RA; ++i) mbar_init(R_FULL(i), 1);
     fence_barrier_init();
   }
   if (a.stats)
@@ -133,73 +171,116 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
 
   if (warp < W_LOAD) {
     // =========================== producers ===========================
-    // One thread = one slab position x all KB channels of the K-block at a time; the (mean, rstd*G, S) rows of the
-    // <= TAB_NB images the tile touches are staged in smem per K-block (double-buffered, one barrier per K-block).
-    const int Cin = a.C0 + a.C1;
+    // One thread = the slab positions h = tid + k * NPROD, all KB channels of the K-block.  The raw input and the
+    // (mean, rstd*G, S) rows of the <= tab_nb images the tile touches arrive by TMA in raw stage g % RA.
     const bool has_tab = a.tab != nullptr;
+    const uint32_t rowb = (uint32_t)a.KB * 4, smask = a.KB == 32 ? 7u : 3u;   // raw row bytes, swizzle row mask
     auto tile_b0_of = [&](int t) {
-      const long long q_first = (long long)(t / groups_n) * MT - a.halo0;
-      return q_first <= 0 ? 0 : (int)min((long long)(a.B - 1), q_first / a.Pimg);
+      const int q_first = (t / groups_n) * MT - a.halo0;
+      return q_first <= 0 ? 0 : min(a.B - 1, q_first / a.Pimg);
     };
+    // TMA issue (thread 0): K-block ikb of work item it, the ig-th K-block of this CTA
+    const uint32_t raw0 = smem_u32(raw_base);
+    const uint32_t main_bytes = (uint32_t)a.nbox * a.boxn * rowb, ctr_bytes = (uint32_t)MT * rowb;
+    const uint32_t tab_bytes = (uint32_t)a.tab_nb * a.KB * (a.tab_planar ? 12 : 16);
+    int it = blockIdx.x, ikb = 0, ig = 0;
+    auto issue_next = [&]() {
+      if (it >= a.ntiles) return;
+      const int p0 = (it / groups_n) * MT;
+      const bool seg2 = ikb >= a.nKB0;
+      int si, cc0;
+      if (!seg2) {
+        const int c0 = ikb * a.KB;
+        if (c0 < a.C0) { si = 0; cc0 = c0; } else { si = 1; cc0 = c0 - a.C0; }
+      } else {
+        const int c0 = (ikb - a.nKB0) * a.KB;
+        if (c0 < a.C2) { si = 2; cc0 = c0; } else { si = 3; cc0 = c0 - a.C2; }
+      }
+      const bool use_tab = has_tab && !seg2;
+      const uint32_t dst = raw0 + (uint32_t)(ig % a.RA) * a.raw_stage;
+      const uint32_t bar = R_FULL(ig % a.RA);
+      mbar_arrive_expect_tx(bar, (seg2 ? ctr_bytes : main_bytes) + (use_tab ? tab_bytes : 0u));
+      if (seg2) {
+        tma_load_2d(dst, &maps.src[si], cc0, first_raw(a, p0), bar);
+      } else {
+        const int r0 = first_raw(a, p0 - a.halo0);
+        for (int i = 0; i < a.nbox; ++i)
+          tma_load_2d(dst + (uint32_t)i * a.boxn * rowb, &maps.src[si], cc0, r0 + i * a.boxn, bar);
+      }
+      if (use_tab) {
+        if (a.tab_planar) tma_load_3d(dst + a.tab_off, &maps.tab, ikb * a.KB, 0, tile_b0_of(it), bar);
+        else tma_load_2d(dst + a.tab_off, &maps.tab, 4 * ikb * a.KB, tile_b0_of(it), bar);
+      }
+      ++ig;
+      if (++ikb == a.nKB) { ikb = 0; it += gridDim.x; }
+    };
+    if (tid == 0)
+      for (int i = 0; i < a.RA - 1; ++i) issue_next();
     int g = 0;                                             // K-blocks produced so far (all tiles)
     for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x) {
-      const long long p0 = (long long)(t / groups_n) * MT;
+      const int p0 = (t / groups_n) * MT;
       const int tb0 = tile_b0_of(t);
+      // per tile, not per K-block: image slot << 16 | row in the first segment's raw box, or -1 for zero padding,
+      // of each position the thread owns (only this thread reads its entries)
+      const int raw_m = first_raw(a, p0 - a.halo0), raw_c = first_raw(a, p0);
+      for (int h = tid; h < a.HP; h += NPROD) {
+        int b = tb0;
+        const int pix = decode_pos(a, p0 - a.halo0 + h, b);
+        pinfo[h] = pix < 0 ? -1 : ((b - tb0) << 16) | (pix - raw_m);
+      }
       for (int kb = 0; kb < a.nKB; ++kb, ++g) {
         const int st = g % a.SA;
-        const float* src; int cs, cc0;
         const bool seg2 = kb >= a.nKB0;
-        if (!seg2) {
-          const int c0 = kb * a.KB;
-          if (c0 < a.C0) { src = a.s0; cs = a.C0; cc0 = c0; } else { src = a.s1; cs = a.C1; cc0 = c0 - a.C0; }
-        } else {
-          const int c0 = (kb - a.nKB0) * a.KB;
-          if (c0 < a.C2) { src = a.s2; cs = a.C2; cc0 = c0; } else { src = a.s3; cs = a.C3; cc0 = c0 - a.C2; }
-        }
         const bool use_tab = has_tab && !seg2;
-        float* tsm = tab_s + (size_t)(g & 1) * TAB_NB * 96;
-        if (use_tab) {
-          for (int i = tid; i < a.tab_nb * a.KB; i += NPROD) {
-            const int bi = i / a.KB, c = i - bi * a.KB;
-            const int b = min(tb0 + bi, a.B - 1);
-            const int ch = kb * a.KB + c;
-            float m, gs, sh;
-            if (a.tab_planar) {
-              const float* tp = a.tab + (long long)b * 3 * Cin + ch;
-              m = __ldg(tp); gs = __ldg(tp + Cin); sh = __ldg(tp + 2 * Cin);
-            } else {
-              const float4 tv = __ldg(reinterpret_cast<const float4*>(a.tab) + (long long)b * Cin + ch);
-              m = tv.x; gs = tv.y * tv.z; sh = tv.w;
-            }
-            tsm[bi * 96 + c] = m; tsm[bi * 96 + 32 + c] = gs; tsm[bi * 96 + 64 + c] = sh;
-          }
-        }
-        mbar_wait(A_EMPTY(st), ((g / a.SA) & 1) ^ 1);
-        // this K-block's table is complete, and every producer finished reading the buffer written two K-blocks ago
+        // the second segment is read at the centre tap only: stage just the tile's own positions, from a box that
+        // starts at the tile's first pixel
+        const int h_lo = seg2 ? a.halo0 : 0, h_hi = seg2 ? a.halo0 + MT : a.HP;
+        const int roff = seg2 ? raw_c - raw_m : 0;
+        // every producer finished reading the raw stage of K-block g - 1: refill it with K-block g + RA - 1
         named_bar_sync(1, NPROD);
+        if (tid == 0) issue_next();
+        mbar_wait(A_EMPTY(st), ((g / a.SA) & 1) ^ 1);
+        const int rs = g % a.RA;
+        mbar_wait(R_FULL(rs), (g / a.RA) & 1);
+        const uint8_t* raw = raw_base + (size_t)rs * a.raw_stage;
+        const float* tsm = reinterpret_cast<const float*>(raw + a.tab_off);
         uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes;
         uint8_t* lo_base = hi_base + a_half_bytes;
+        const int h0 = h_lo + (tid - h_lo % NPROD + NPROD) % NPROD;   // first owned position >= h_lo
 #pragma unroll 1
-        for (int h = tid; h < a.HP; h += NPROD) {
-          int b = tb0;
-          const int pix = decode_pos(a, p0 - a.halo0 + h, b);
-          const int bidx = b - tb0;
-          float4 raw[8];
+        for (int h = h0; h < h_hi; h += NPROD) {
+          const int info = pinfo[h];
+          const bool pad = info < 0;
+          const int bidx = info >> 16;
+          const uint32_t row = (uint32_t)((info & 0xffff) - roff);
+          float4 rv[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            if (j < 2 * chunks) raw[j] = pix >= 0 ? __ldg(reinterpret_cast<const float4*>(src + (long long)pix * cs + cc0) + j)
-                                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+            if (j < 2 * chunks) {
+              const uint32_t off = row * rowb + 16u * j;
+              rv[j] = pad ? make_float4(0.f, 0.f, 0.f, 0.f)
+                          : *reinterpret_cast<const float4*>(raw + (off ^ (((off >> 7) & smask) << 4)));
+            }
 #pragma unroll
           for (int ch = 0; ch < 4; ++ch) {
             if (ch < chunks) {
               uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
-              if (pix >= 0) {
-                float v[8] = {raw[2 * ch].x, raw[2 * ch].y, raw[2 * ch].z, raw[2 * ch].w,
-                              raw[2 * ch + 1].x, raw[2 * ch + 1].y, raw[2 * ch + 1].z, raw[2 * ch + 1].w};
+              if (!pad) {
+                float v[8] = {rv[2 * ch].x, rv[2 * ch].y, rv[2 * ch].z, rv[2 * ch].w,
+                              rv[2 * ch + 1].x, rv[2 * ch + 1].y, rv[2 * ch + 1].z, rv[2 * ch + 1].w};
                 if (use_tab) {
-                  const float* tb = tsm + bidx * 96 + ch * 8;
+                  if (a.tab_planar) {                      // [tab_nb][mean | rstd*G | S][KB]
+                    const float* tb = tsm + bidx * 3 * a.KB + ch * 8;
 #pragma unroll
-                  for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tb[e], tb[32 + e], tb[64 + e]);
+                    for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tb[e], tb[a.KB + e], tb[2 * a.KB + e]);
+                  } else {                                 // [tab_nb][KB] float4 (mean, rstd, G, S)
+                    const float4* tb = reinterpret_cast<const float4*>(tsm) + bidx * a.KB + ch * 8;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                      const float4 tv = tb[e];
+                      v[e] = fmaf(v[e] - tv.x, tv.y * tv.z, tv.w);
+                    }
+                  }
                   if (a.act_in) silu_fast8(v);
                 }
                 uint32_t hw[4], lw[4];
@@ -251,7 +332,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
     int bst = 0, bph = 0, g0 = 0;                          // g0: first K-block (all items) of the current item
     for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x, g0 += a.nKB)
      for (int j = 0; j < a.NPI; ++j) {
-      const long long p0 = (long long)(t / groups_n) * MT;
+      const int p0 = (t / groups_n) * MT;
       const int n0 = ((t % groups_n) * a.NPI + j) * NT;
       const bool last_n = j == a.NPI - 1;                  // the slab stages are released after the item's last n tile
       float acc[NT / 2];
@@ -299,7 +380,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a) {
       const int r0 = 64 * wg + 16 * wq + (lane >> 2);
       const int cq = 2 * (lane & 3);
       int pix[2], slot[2];
-      const int tile_b0 = (int)min((long long)(a.B - 1), p0 / a.Pimg);
+      const int tile_b0 = min(a.B - 1, p0 / a.Pimg);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         int b = 0;
@@ -418,12 +499,17 @@ int conv_kb(int C0, int C1, int C2, int C3) {
 
 struct Plan {
   int HP, NB, NJ;
+  int boxn, nbox, tab_nb;   // first-segment TMA boxes; images whose norm-table rows a raw stage holds
+  int raw_off, raw_stage, tab_off, RA;
   size_t smem;
 };
 
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 
-// shared-memory plan of one conv with SA slab stages; false when it does not fit
+size_t round1024(size_t x) { return (x + 1023) & ~(size_t)1023; }
+
+// shared-memory plan of one conv with SA slab stages (two raw stages where they fit); false when it does not fit.  Layout: slab stages, weight
+// stages, raw stages (1024-byte aligned for the swizzled TMA boxes), position table, statistics, barriers.
 bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, Plan& p) {
   const int Wp = ks == 3 ? W + 1 : W;
   const int Pimg = ks == 3 ? (H + 1) * (W + 1) : H * W;
@@ -431,22 +517,70 @@ bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, Plan& p
   p.HP = (MT + 2 * halo0 + 7) & ~7;
   p.NJ = (MT - 1) / Pimg + 2;
   if (p.HP > HP_MAX) return false;
+  p.nbox = p.HP > 256 ? 2 : 1;                               // TMA boxes hold <= 256 rows
+  p.boxn = p.nbox == 1 ? p.HP : ((p.HP / 2 + 7) & ~7);      // a multiple of 8 rows keeps box 2 swizzle-aligned
+  p.tab_nb = std::min(p.HP / Pimg + 2, TAB_NB);
+  p.tab_off = p.nbox * p.boxn * KB * 4;
+  p.raw_stage = (int)round1024((size_t)p.tab_off + (size_t)p.tab_nb * KB * 16);
   const size_t a_stage = (size_t)2 * (KB / 8) * p.HP * 16;
   const size_t b_stage = (size_t)(KB / 16) * 64 * NT;
   const size_t stat_bytes = stats ? (size_t)p.NJ * 2 * NT * 8 : 0;
-  const size_t fixed = SA * a_stage + (size_t)2 * TAB_NB * 96 * 4 + stat_bytes + 8 * (2 * SA + 20);   // ... + barriers
-  if (fixed + 2 * b_stage > SMEM_LIMIT) return false;
+  const size_t pinfo_bytes = (size_t)PPT * NPROD * 4;
+  size_t bar_bytes = 0, fixed = 0;
+  for (p.RA = RAW_STAGES; p.RA >= 1; --p.RA) {
+    bar_bytes = 8 * (2 * SA + 20 + p.RA);
+    fixed = round1024(SA * a_stage) + (size_t)p.RA * p.raw_stage + pinfo_bytes + stat_bytes + bar_bytes;
+    if (fixed + 2 * b_stage <= SMEM_LIMIT) break;
+  }
+  if (p.RA == 0) return false;
   p.NB = (int)((SMEM_LIMIT - fixed) / b_stage);
   if (p.NB > 10) p.NB = 10;
-  p.smem = fixed + (size_t)p.NB * b_stage;
-  return true;
+  p.raw_off = (int)round1024(SA * a_stage + (size_t)p.NB * b_stage);
+  p.smem = (size_t)p.raw_off + (size_t)p.RA * p.raw_stage + pinfo_bytes + stat_bytes + bar_bytes;
+  return p.smem <= SMEM_LIMIT;
+}
+
+using EncodeTiled = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                 const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                 CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// cuTensorMapEncodeTiled from the driver the runtime already loaded (the library does not link libcuda)
+EncodeTiled encode_tiled() {
+  static const EncodeTiled fn = [] {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      f = nullptr;
+    return reinterpret_cast<EncodeTiled>(f);
+  }();
+  return fn;
+}
+
+// tiled map of an fp32 tensor (dims innermost first, byte strides of dims 1..rank-1); zero fill out of range
+int encode_map(CUtensorMap* m, const float* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+               const cuuint32_t* box, CUtensorMapSwizzle swz, const char* name) {
+  MCVD_CHECK(((uintptr_t)base & 15) == 0, "%s: TMA source %p is not 16-byte aligned", name, (const void*)base);
+  for (int i = 0; i < rank; ++i)
+    MCVD_CHECK(box[i] >= 1 && box[i] <= 256, "%s: TMA box dimension %u outside [1, 256]", name, box[i]);
+  for (int i = 0; i < rank - 1; ++i)
+    MCVD_CHECK(strides[i] % 16 == 0, "%s: TMA stride %llu bytes is not a multiple of 16", name,
+               (unsigned long long)strides[i]);
+  const EncodeTiled enc = encode_tiled();
+  MCVD_CHECK(enc != nullptr, "%s: cuTensorMapEncodeTiled unavailable", name);
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<float*>(base), dims, strides,
+                         box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MCVD_CHECK(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed (%d)", name, (int)r);
+  return 0;
 }
 
 template <int NT>
-int launch_nt(const ConvArgs& a, size_t smem, int grid, cudaStream_t s) {
+int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, cudaStream_t s) {
   cudaError_t e = cudaFuncSetAttribute(k_conv_umma<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   MCVD_CHECK(e == cudaSuccess, "CONV_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-  k_conv_umma<NT><<<grid, NTHREADS, smem, s>>>(a);
+  k_conv_umma<NT><<<grid, NTHREADS, smem, s>>>(a, m);
   MCVD_CUDA_LAUNCH_CHECK("conv_umma");
   return 0;
 }
@@ -474,8 +608,8 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
              op.Cout);
   if (a.ks == 3) { a.Wp = op.W + 1; a.Pimg = (op.H + 1) * (op.W + 1); }
   else { a.Wp = op.W; a.Pimg = op.H * op.W; }
-  a.Qtot = (long long)op.B * a.Pimg;
-  MCVD_CHECK((long long)op.B * op.H * op.W < (1LL << 31) && a.Qtot < (1LL << 31), "%s: too many pixels", name);
+  MCVD_CHECK((long long)op.B * a.Pimg < (1LL << 31), "%s: too many pixels", name);
+  a.Qtot = op.B * a.Pimg;
   MCVD_CHECK(!a.stats || a.Pimg >= 64, "%s: epilogue statistics need images of >= 64 positions", name);
   a.halo0 = (a.ks == 3) ? a.Wp + 1 : 0;
   a.nKB0 = (op.C0 + op.C1) / a.KB;
@@ -505,6 +639,8 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, p),
              "%s: tile does not fit shared memory (W=%d)", name, op.W);
   a.HP = p.HP; a.NB = p.NB; a.NJ = p.NJ;
+  a.boxn = p.boxn; a.nbox = p.nbox; a.raw_off = p.raw_off; a.raw_stage = p.raw_stage; a.tab_off = p.tab_off;
+  a.RA = p.RA;
   a.act_in = (op.flags & MCVD_F_ACT_IN) ? 1 : 0;
   a.act_out = (op.flags & MCVD_F_ACT_OUT) ? 1 : 0;
   a.wscale = op.f1; a.oscale = op.f0;
@@ -514,11 +650,41 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
     MCVD_CHECK(nb <= TAB_NB || !a.tab, "%s: %dx%d images are too small for the fused-norm path", name, op.H, op.W);
     a.tab_nb = (nb <= TAB_NB) ? nb : 0;
   }
+  // TMA maps: sources as {C, B*H*W} rows of KB channels, swizzled; the norm table as {4*Cin, B} or {Cin, 3, B}
+  ConvMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  {
+    const float* srcs[4] = {a.s0, a.s1, a.s2, a.s3};
+    const int cs[4] = {a.C0, a.C1, a.C2, a.C3};
+    const CUtensorMapSwizzle swz = a.KB == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    for (int i = 0; i < 4; ++i) {
+      if (!cs[i]) continue;
+      MCVD_CHECK(srcs[i] != nullptr, "%s: null source %d", name, i);
+      const cuuint64_t dims[2] = {(cuuint64_t)cs[i], (cuuint64_t)op.B * op.H * op.W};
+      const cuuint64_t strides[1] = {(cuuint64_t)cs[i] * 4};
+      const cuuint32_t box[2] = {(cuuint32_t)a.KB, (cuuint32_t)(i < 2 ? a.boxn : MT)};
+      if (encode_map(&maps.src[i], srcs[i], 2, dims, strides, box, swz, name)) return -1;
+    }
+    if (a.tab) {
+      const int Cin = op.C0 + op.C1;
+      if (planar) {
+        const cuuint64_t dims[3] = {(cuuint64_t)Cin, 3, (cuuint64_t)op.B};
+        const cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)Cin * 12};
+        const cuuint32_t box[3] = {(cuuint32_t)a.KB, 3, (cuuint32_t)a.tab_nb};
+        if (encode_map(&maps.tab, a.tab, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE, name)) return -1;
+      } else {
+        const cuuint64_t dims[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)op.B};
+        const cuuint64_t strides[1] = {(cuuint64_t)Cin * 16};
+        const cuuint32_t box[2] = {(cuuint32_t)(4 * a.KB), (cuuint32_t)a.tab_nb};
+        if (encode_map(&maps.tab, a.tab, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE, name)) return -1;
+      }
+    }
+  }
   MCVD_CHECK(tiles_m * a.tiles_n < (1LL << 31), "%s: too many tiles", name);
   a.ntiles = (int)(tiles_m * (a.tiles_n / a.NPI));
   const int grid = a.ntiles < sms ? a.ntiles : sms;
   switch (NT) {
-#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, p.smem, grid, s);
+#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, maps, p.smem, grid, s);
     MCVD_NT_CASE(16) MCVD_NT_CASE(32) MCVD_NT_CASE(48) MCVD_NT_CASE(64) MCVD_NT_CASE(80) MCVD_NT_CASE(96)
     MCVD_NT_CASE(112) MCVD_NT_CASE(128) MCVD_NT_CASE(144) MCVD_NT_CASE(160) MCVD_NT_CASE(176) MCVD_NT_CASE(192)
     MCVD_NT_CASE(208) MCVD_NT_CASE(224) MCVD_NT_CASE(240) MCVD_NT_CASE(256)
@@ -574,7 +740,7 @@ extern "C" int mcvd_umma2_plan(int H, int W, int ks, int C0, int C1, int C2, int
   return mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, p) ? kb : 0;
 }
 
-// shared-memory plan of a conv (diagnostics / tests): out[0..9] = KB, HP, image stages, raw-ring stages (0), weight
+// shared-memory plan of a conv (diagnostics / tests): out[0..9] = KB, HP, image stages, raw-input stages, weight
 // stages, image slots per tile, accumulator columns outside registers (0), dynamic shared memory bytes, tiles
 // per unit (1), accumulator sets (1); returns 0, or -1
 extern "C" int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats,
@@ -583,7 +749,7 @@ extern "C" int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2
   if (!kb || !out) return -1;
   mcvd::Plan p;
   mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, p);
-  out[0] = kb; out[1] = p.HP; out[2] = 2; out[3] = 0; out[4] = p.NB; out[5] = p.NJ; out[6] = 0;
+  out[0] = kb; out[1] = p.HP; out[2] = 2; out[3] = p.RA; out[4] = p.NB; out[5] = p.NJ; out[6] = 0;
   out[7] = (int)p.smem; out[8] = 1; out[9] = 1;
   return 0;
 }
