@@ -22,19 +22,24 @@
 //     [k-chunk of 8 halfs][position][8 halfs = 16 B]      LBO = positions*16 B,  SBO = 128 B.
 // Outputs at padding positions are computed and discarded (2..20 % of the rows).
 //
-// Warp roles (384 threads, one CTA per SM, persistent over 128-position x NT tiles):
+// Warp roles (128 * (NWG + 1) threads, one CTA per SM, persistent over MT x NT tiles, MT = 64 * NWG positions):
 //   warps 0-2   producers: raw fp32 NHWC stage in smem -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2 stages)
 //               (generic-proxy stores + fence.proxy.async).  Thread 0 also issues the TMA (cp.async.bulk.tensor)
 //               loads of the raw input boxes and norm-table rows, one K-block ahead of the conversion.
 //   warp  3     weight loader: cp.async.bulk (TMA 1-D) of pre-packed fp16 hi/lo smem images (ring of NB stages)
-//   warps 4-11  two consumer warpgroups, 64 rows of the tile each: wgmma m64nNTk16 from the slab and weight
+//   warps 4-    NWG = 2 or 3 consumer warpgroups, 64 rows of the tile each: wgmma m64nNTk16 from the slab and weight
 //               stages, then the epilogue straight from the accumulator registers (bias / residual / scale /
 //               SiLU, optional GroupNorm statistics of the stored output)
+// Tile height.  The weight bytes streamed per MMA and the halo positions converted per output position both fall
+// as 1/MT, so streaming convs with NT <= 192 run three consumer warpgroups (MT = 192): warpgroup 0 gives registers
+// back (setmaxnreg) so that the consumers hold 96 accumulators each.  Statistics-writing and input-stationary
+// launches keep MT = 128 (their statistics layout and slab stages are sized in 128-position tiles).  Every output
+// sums the same products in the same order at either height, so the two give identical bits.
 //
 // Raw input stages.  The real pixels among consecutive padded-flat positions are consecutive NHWC pixels, so the
 // raw input of a slab is one run of rows of a 2-D {C_src, B*H*W} tensor map: one TMA box of HP rows (two when
 // HP > 256, the box-size limit), zero-filled past the end of the batch.  One-tap K-blocks (1x1 convs, the fused
-// shortcut segment) load and convert only the 128 rows of the tile's own positions.  The boxes are 64- / 128-byte
+// shortcut segment) load and convert only the MT rows of the tile's own positions.  The boxes are 64- / 128-byte
 // swizzled (KB = 16 / 32 channels per row) so that eight producers reading the same 16 bytes of eight consecutive
 // rows hit distinct banks.
 #include <cuda.h>
@@ -48,7 +53,7 @@
 
 namespace mcvd {
 
-constexpr int MT = 128;         // positions per tile (two consumer warpgroups x 64)
+constexpr int STAT_MT = 128;    // positions per tile of the statistics layout (the two-warpgroup tile)
 
 namespace {
 
@@ -56,11 +61,15 @@ using namespace ptx;
 
 constexpr int NPROD = 96;       // producer threads (warps 0-2)
 constexpr int W_LOAD = 3;       // weight-loader warp
-constexpr int W_CONS = 4;       // first consumer warp (warpgroups 1 and 2)
-constexpr int NTHREADS = 384;   // 168 registers per thread: room for the 128 accumulators of NT = 256
+constexpr int W_CONS = 4;       // first consumer warp (warpgroups 1..NWG)
+// NWG = 2: 384 threads, 168 registers each: room for the 128 accumulators of NT = 256.  NWG = 3: 512 threads launched
+// at 128 registers; warpgroup 0 drops to 96 and the consumers rise to 136 (128 * 96 + 384 * 136 <= 65536), enough
+// for the 96 accumulators of NT = 192 without spills (the producers spill below 88)
+constexpr int NT_MAX3 = 192;
+constexpr int REG_PROD3 = 96, REG_CONS3 = 136;
 constexpr float STAT_SCALE = 65536.0f;   // fixed-point scale of the epilogue statistics
 constexpr int TAB_NB = 8;       // images whose norm-table rows are staged in smem per K-block
-constexpr int HP_MAX = 512;
+constexpr int HP_MAX = 512;     // >= 192 + 2 * 130 rounded to 8 = 456, the MT = 192 slab at 128x128
 constexpr int PPT = (HP_MAX + NPROD - 1) / NPROD;   // slab positions per producer thread
 constexpr int RAW_STAGES = 2;   // raw input stages: the loads of K-block g + 1 fly while K-block g is converted
 constexpr int MAX_RESIDENT = 12;   // K-blocks an input-stationary work item keeps resident (12 x 16 KB at KB = 32)
@@ -132,8 +141,13 @@ __device__ __forceinline__ int first_raw(const ConvArgs& a, int q) {
   return (b * a.H + (rr - 1)) * a.W + (cc == 0 ? 0 : cc - 1);
 }
 
-template <int NT>
-__global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a, const __grid_constant__ ConvMaps maps) {
+template <int NT, int NWG>
+__global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs a,
+                                                                  const __grid_constant__ ConvMaps maps) {
+  static_assert(NWG == 2 || (NWG == 3 && NT <= NT_MAX3), "three consumer warpgroups hold at most 96 accumulators");
+  constexpr int MT = 64 * NWG;                                       // positions per tile
+  constexpr int NTHREADS = 128 * (NWG + 1);
+  constexpr int NCONS = 4 * NWG;                                     // consumer warps
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int chunks = a.KB / 8;
   const uint32_t a_half_bytes = (uint32_t)chunks * a.HP * 16;       // one of hi / lo
@@ -159,9 +173,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a, con
   const int taps = a.ks * a.ks;
 
   if (tid == 0) {
-    // consumers release a stage with one arrival per consumer warp (8)
-    for (int i = 0; i < a.SA; ++i) { mbar_init(A_FULL(i), NPROD); mbar_init(A_EMPTY(i), 8); }
-    for (int i = 0; i < a.NB; ++i) { mbar_init(B_FULL(i), 1); mbar_init(B_EMPTY(i), 8); }
+    // consumers release a stage with one arrival per consumer warp
+    for (int i = 0; i < a.SA; ++i) { mbar_init(A_FULL(i), NPROD); mbar_init(A_EMPTY(i), NCONS); }
+    for (int i = 0; i < a.NB; ++i) { mbar_init(B_FULL(i), 1); mbar_init(B_EMPTY(i), NCONS); }
     for (int i = 0; i < a.RA; ++i) mbar_init(R_FULL(i), 1);
     fence_barrier_init();
   }
@@ -169,156 +183,162 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a, con
     for (int i = tid; i < a.NJ * 2 * NT; i += NTHREADS) stat_s[i] = 0ull;
   __syncthreads();
 
-  if (warp < W_LOAD) {
-    // =========================== producers ===========================
-    // One thread = the slab positions h = tid + k * NPROD, all KB channels of the K-block.  The raw input and the
-    // (mean, rstd*G, S) rows of the <= tab_nb images the tile touches arrive by TMA in raw stage g % RA.
-    const bool has_tab = a.tab != nullptr;
-    const uint32_t rowb = (uint32_t)a.KB * 4, smask = a.KB == 32 ? 7u : 3u;   // raw row bytes, swizzle row mask
-    auto tile_b0_of = [&](int t) {
-      const int q_first = (t / groups_n) * MT - a.halo0;
-      return q_first <= 0 ? 0 : min(a.B - 1, q_first / a.Pimg);
-    };
-    // TMA issue (thread 0): K-block ikb of work item it, the ig-th K-block of this CTA
-    const uint32_t raw0 = smem_u32(raw_base);
-    const uint32_t main_bytes = (uint32_t)a.nbox * a.boxn * rowb, ctr_bytes = (uint32_t)MT * rowb;
-    const uint32_t tab_bytes = (uint32_t)a.tab_nb * a.KB * (a.tab_planar ? 12 : 16);
-    int it = blockIdx.x, ikb = 0, ig = 0;
-    auto issue_next = [&]() {
-      if (it >= a.ntiles) return;
-      const int p0 = (it / groups_n) * MT;
-      const bool seg2 = ikb >= a.nKB0;
-      int si, cc0;
-      if (!seg2) {
-        const int c0 = ikb * a.KB;
-        if (c0 < a.C0) { si = 0; cc0 = c0; } else { si = 1; cc0 = c0 - a.C0; }
-      } else {
-        const int c0 = (ikb - a.nKB0) * a.KB;
-        if (c0 < a.C2) { si = 2; cc0 = c0; } else { si = 3; cc0 = c0 - a.C2; }
-      }
-      const bool use_tab = has_tab && !seg2;
-      const uint32_t dst = raw0 + (uint32_t)(ig % a.RA) * a.raw_stage;
-      const uint32_t bar = R_FULL(ig % a.RA);
-      mbar_arrive_expect_tx(bar, (seg2 ? ctr_bytes : main_bytes) + (use_tab ? tab_bytes : 0u));
-      if (seg2) {
-        tma_load_2d(dst, &maps.src[si], cc0, first_raw(a, p0), bar);
-      } else {
-        const int r0 = first_raw(a, p0 - a.halo0);
-        for (int i = 0; i < a.nbox; ++i)
-          tma_load_2d(dst + (uint32_t)i * a.boxn * rowb, &maps.src[si], cc0, r0 + i * a.boxn, bar);
-      }
-      if (use_tab) {
-        if (a.tab_planar) tma_load_3d(dst + a.tab_off, &maps.tab, ikb * a.KB, 0, tile_b0_of(it), bar);
-        else tma_load_2d(dst + a.tab_off, &maps.tab, 4 * ikb * a.KB, tile_b0_of(it), bar);
-      }
-      ++ig;
-      if (++ikb == a.nKB) { ikb = 0; it += gridDim.x; }
-    };
-    if (tid == 0)
-      for (int i = 0; i < a.RA - 1; ++i) issue_next();
-    int g = 0;                                             // K-blocks produced so far (all tiles)
-    for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x) {
-      const int p0 = (t / groups_n) * MT;
-      const int tb0 = tile_b0_of(t);
-      // per tile, not per K-block: image slot << 16 | row in the first segment's raw box, or -1 for zero padding,
-      // of each position the thread owns (only this thread reads its entries)
-      const int raw_m = first_raw(a, p0 - a.halo0), raw_c = first_raw(a, p0);
-      for (int h = tid; h < a.HP; h += NPROD) {
-        int b = tb0;
-        const int pix = decode_pos(a, p0 - a.halo0 + h, b);
-        pinfo[h] = pix < 0 ? -1 : ((b - tb0) << 16) | (pix - raw_m);
-      }
-      for (int kb = 0; kb < a.nKB; ++kb, ++g) {
-        const int st = g % a.SA;
-        const bool seg2 = kb >= a.nKB0;
+  if (warp < W_CONS) {
+    // warpgroup 0 (producers and weight loader) hands registers to the consumers; the branch structure lets ptxas
+    // allocate each role within its budget
+    if constexpr (NWG == 3) setmaxnreg_dec<REG_PROD3>();
+    if (warp < W_LOAD) {
+      // =========================== producers ===========================
+      // One thread = the slab positions h = tid + k * NPROD, all KB channels of the K-block.  The raw input and the
+      // (mean, rstd*G, S) rows of the <= tab_nb images the tile touches arrive by TMA in raw stage g % RA.
+      const bool has_tab = a.tab != nullptr;
+      const uint32_t rowb = (uint32_t)a.KB * 4, smask = a.KB == 32 ? 7u : 3u;   // raw row bytes, swizzle row mask
+      auto tile_b0_of = [&](int t) {
+        const int q_first = (t / groups_n) * MT - a.halo0;
+        return q_first <= 0 ? 0 : min(a.B - 1, q_first / a.Pimg);
+      };
+      // TMA issue (thread 0): K-block ikb of work item it, the ig-th K-block of this CTA
+      const uint32_t raw0 = smem_u32(raw_base);
+      const uint32_t main_bytes = (uint32_t)a.nbox * a.boxn * rowb, ctr_bytes = (uint32_t)MT * rowb;
+      const uint32_t tab_bytes = (uint32_t)a.tab_nb * a.KB * (a.tab_planar ? 12 : 16);
+      int it = blockIdx.x, ikb = 0, ig = 0;
+      auto issue_next = [&]() {
+        if (it >= a.ntiles) return;
+        const int p0 = (it / groups_n) * MT;
+        const bool seg2 = ikb >= a.nKB0;
+        int si, cc0;
+        if (!seg2) {
+          const int c0 = ikb * a.KB;
+          if (c0 < a.C0) { si = 0; cc0 = c0; } else { si = 1; cc0 = c0 - a.C0; }
+        } else {
+          const int c0 = (ikb - a.nKB0) * a.KB;
+          if (c0 < a.C2) { si = 2; cc0 = c0; } else { si = 3; cc0 = c0 - a.C2; }
+        }
         const bool use_tab = has_tab && !seg2;
-        // the second segment is read at the centre tap only: stage just the tile's own positions, from a box that
-        // starts at the tile's first pixel
-        const int h_lo = seg2 ? a.halo0 : 0, h_hi = seg2 ? a.halo0 + MT : a.HP;
-        const int roff = seg2 ? raw_c - raw_m : 0;
-        // every producer finished reading the raw stage of K-block g - 1: refill it with K-block g + RA - 1
-        named_bar_sync(1, NPROD);
-        if (tid == 0) issue_next();
-        mbar_wait(A_EMPTY(st), ((g / a.SA) & 1) ^ 1);
-        const int rs = g % a.RA;
-        mbar_wait(R_FULL(rs), (g / a.RA) & 1);
-        const uint8_t* raw = raw_base + (size_t)rs * a.raw_stage;
-        const float* tsm = reinterpret_cast<const float*>(raw + a.tab_off);
-        uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes;
-        uint8_t* lo_base = hi_base + a_half_bytes;
-        const int h0 = h_lo + (tid - h_lo % NPROD + NPROD) % NPROD;   // first owned position >= h_lo
+        const uint32_t dst = raw0 + (uint32_t)(ig % a.RA) * a.raw_stage;
+        const uint32_t bar = R_FULL(ig % a.RA);
+        mbar_arrive_expect_tx(bar, (seg2 ? ctr_bytes : main_bytes) + (use_tab ? tab_bytes : 0u));
+        if (seg2) {
+          tma_load_2d(dst, &maps.src[si], cc0, first_raw(a, p0), bar);
+        } else {
+          const int r0 = first_raw(a, p0 - a.halo0);
+          for (int i = 0; i < a.nbox; ++i)
+            tma_load_2d(dst + (uint32_t)i * a.boxn * rowb, &maps.src[si], cc0, r0 + i * a.boxn, bar);
+        }
+        if (use_tab) {
+          if (a.tab_planar) tma_load_3d(dst + a.tab_off, &maps.tab, ikb * a.KB, 0, tile_b0_of(it), bar);
+          else tma_load_2d(dst + a.tab_off, &maps.tab, 4 * ikb * a.KB, tile_b0_of(it), bar);
+        }
+        ++ig;
+        if (++ikb == a.nKB) { ikb = 0; it += gridDim.x; }
+      };
+      if (tid == 0)
+        for (int i = 0; i < a.RA - 1; ++i) issue_next();
+      int g = 0;                                             // K-blocks produced so far (all tiles)
+      for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x) {
+        const int p0 = (t / groups_n) * MT;
+        const int tb0 = tile_b0_of(t);
+        // per tile, not per K-block: image slot << 16 | row in the first segment's raw box, or -1 for zero padding,
+        // of each position the thread owns (only this thread reads its entries)
+        const int raw_m = first_raw(a, p0 - a.halo0), raw_c = first_raw(a, p0);
+        for (int h = tid; h < a.HP; h += NPROD) {
+          int b = tb0;
+          const int pix = decode_pos(a, p0 - a.halo0 + h, b);
+          pinfo[h] = pix < 0 ? -1 : ((b - tb0) << 16) | (pix - raw_m);
+        }
+        for (int kb = 0; kb < a.nKB; ++kb, ++g) {
+          const int st = g % a.SA;
+          const bool seg2 = kb >= a.nKB0;
+          const bool use_tab = has_tab && !seg2;
+          // the second segment is read at the centre tap only: stage just the tile's own positions, from a box that
+          // starts at the tile's first pixel
+          const int h_lo = seg2 ? a.halo0 : 0, h_hi = seg2 ? a.halo0 + MT : a.HP;
+          const int roff = seg2 ? raw_c - raw_m : 0;
+          // every producer finished reading the raw stage of K-block g - 1: refill it with K-block g + RA - 1
+          named_bar_sync(1, NPROD);
+          if (tid == 0) issue_next();
+          mbar_wait(A_EMPTY(st), ((g / a.SA) & 1) ^ 1);
+          const int rs = g % a.RA;
+          mbar_wait(R_FULL(rs), (g / a.RA) & 1);
+          const uint8_t* raw = raw_base + (size_t)rs * a.raw_stage;
+          const float* tsm = reinterpret_cast<const float*>(raw + a.tab_off);
+          uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes;
+          uint8_t* lo_base = hi_base + a_half_bytes;
+          const int h0 = h_lo + (tid - h_lo % NPROD + NPROD) % NPROD;   // first owned position >= h_lo
 #pragma unroll 1
-        for (int h = h0; h < h_hi; h += NPROD) {
-          const int info = pinfo[h];
-          const bool pad = info < 0;
-          const int bidx = info >> 16;
-          const uint32_t row = (uint32_t)((info & 0xffff) - roff);
-          float4 rv[8];
+          for (int h = h0; h < h_hi; h += NPROD) {
+            const int info = pinfo[h];
+            const bool pad = info < 0;
+            const int bidx = info >> 16;
+            const uint32_t row = (uint32_t)((info & 0xffff) - roff);
+            float4 rv[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (j < 2 * chunks) {
-              const uint32_t off = row * rowb + 16u * j;
-              rv[j] = pad ? make_float4(0.f, 0.f, 0.f, 0.f)
-                          : *reinterpret_cast<const float4*>(raw + (off ^ (((off >> 7) & smask) << 4)));
-            }
-#pragma unroll
-          for (int ch = 0; ch < 4; ++ch) {
-            if (ch < chunks) {
-              uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
-              if (!pad) {
-                float v[8] = {rv[2 * ch].x, rv[2 * ch].y, rv[2 * ch].z, rv[2 * ch].w,
-                              rv[2 * ch + 1].x, rv[2 * ch + 1].y, rv[2 * ch + 1].z, rv[2 * ch + 1].w};
-                if (use_tab) {
-                  if (a.tab_planar) {                      // [tab_nb][mean | rstd*G | S][KB]
-                    const float* tb = tsm + bidx * 3 * a.KB + ch * 8;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tb[e], tb[a.KB + e], tb[2 * a.KB + e]);
-                  } else {                                 // [tab_nb][KB] float4 (mean, rstd, G, S)
-                    const float4* tb = reinterpret_cast<const float4*>(tsm) + bidx * a.KB + ch * 8;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                      const float4 tv = tb[e];
-                      v[e] = fmaf(v[e] - tv.x, tv.y * tv.z, tv.w);
-                    }
-                  }
-                  if (a.act_in) silu_fast8(v);
-                }
-                uint32_t hw[4], lw[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
-                hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+            for (int j = 0; j < 8; ++j)
+              if (j < 2 * chunks) {
+                const uint32_t off = row * rowb + 16u * j;
+                rv[j] = pad ? make_float4(0.f, 0.f, 0.f, 0.f)
+                            : *reinterpret_cast<const float4*>(raw + (off ^ (((off >> 7) & smask) << 4)));
               }
-              const size_t off = ((size_t)ch * a.HP + h) * 16;
-              *reinterpret_cast<uint4*>(hi_base + off) = hv;
-              *reinterpret_cast<uint4*>(lo_base + off) = lv;
+#pragma unroll
+            for (int ch = 0; ch < 4; ++ch) {
+              if (ch < chunks) {
+                uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
+                if (!pad) {
+                  float v[8] = {rv[2 * ch].x, rv[2 * ch].y, rv[2 * ch].z, rv[2 * ch].w,
+                                rv[2 * ch + 1].x, rv[2 * ch + 1].y, rv[2 * ch + 1].z, rv[2 * ch + 1].w};
+                  if (use_tab) {
+                    if (a.tab_planar) {                      // [tab_nb][mean | rstd*G | S][KB]
+                      const float* tb = tsm + bidx * 3 * a.KB + ch * 8;
+#pragma unroll
+                      for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tb[e], tb[a.KB + e], tb[2 * a.KB + e]);
+                    } else {                                 // [tab_nb][KB] float4 (mean, rstd, G, S)
+                      const float4* tb = reinterpret_cast<const float4*>(tsm) + bidx * a.KB + ch * 8;
+#pragma unroll
+                      for (int e = 0; e < 8; ++e) {
+                        const float4 tv = tb[e];
+                        v[e] = fmaf(v[e] - tv.x, tv.y * tv.z, tv.w);
+                      }
+                    }
+                    if (a.act_in) silu_fast8(v);
+                  }
+                  uint32_t hw[4], lw[4];
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
+                  hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+                  lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                }
+                const size_t off = ((size_t)ch * a.HP + h) * 16;
+                *reinterpret_cast<uint4*>(hi_base + off) = hv;
+                *reinterpret_cast<uint4*>(lo_base + off) = lv;
+              }
             }
           }
-        }
-        fence_proxy_async();          // make the generic-proxy stores visible to the tensor-core (async) proxy
-        mbar_arrive(A_FULL(st));
-      }
-    }
-  } else if (warp == W_LOAD) {
-    // =========================== weight loader ===========================
-    if (elect_one()) {
-      const uint32_t b0 = smem_u32(b_base);
-      const int per_tile = a.nKB0 * taps + (a.nKB - a.nKB0);          // second segment: one (centre) tap per K-block
-      int st = 0, ph = 1;
-      for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x)
-       for (int j = 0; j < a.NPI; ++j) {
-        const int nt = (t % groups_n) * a.NPI + j;
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wpk) + (size_t)nt * per_tile * b_stage_bytes;
-        for (int i = 0; i < per_tile; ++i) {
-          mbar_wait(B_EMPTY(st), ph);
-          mbar_arrive_expect_tx(B_FULL(st), b_stage_bytes);
-          bulk_g2s(b0 + (uint32_t)st * b_stage_bytes, wsrc + (size_t)i * b_stage_bytes, b_stage_bytes, B_FULL(st));
-          if (++st == a.NB) { st = 0; ph ^= 1; }
+          fence_proxy_async();          // make the generic-proxy stores visible to the tensor-core (async) proxy
+          mbar_arrive(A_FULL(st));
         }
       }
+    } else if (warp == W_LOAD) {
+      // =========================== weight loader ===========================
+      if (elect_one()) {
+        const uint32_t b0 = smem_u32(b_base);
+        const int per_tile = a.nKB0 * taps + (a.nKB - a.nKB0);          // second segment: one (centre) tap per K-block
+        int st = 0, ph = 1;
+        for (int t = blockIdx.x; t < a.ntiles; t += gridDim.x)
+         for (int j = 0; j < a.NPI; ++j) {
+          const int nt = (t % groups_n) * a.NPI + j;
+          const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wpk) + (size_t)nt * per_tile * b_stage_bytes;
+          for (int i = 0; i < per_tile; ++i) {
+            mbar_wait(B_EMPTY(st), ph);
+            mbar_arrive_expect_tx(B_FULL(st), b_stage_bytes);
+            bulk_g2s(b0 + (uint32_t)st * b_stage_bytes, wsrc + (size_t)i * b_stage_bytes, b_stage_bytes, B_FULL(st));
+            if (++st == a.NB) { st = 0; ph ^= 1; }
+          }
+        }
+      }
+      __syncwarp();
     }
-    __syncwarp();
   } else {
+    if constexpr (NWG == 3) setmaxnreg_inc<REG_CONS3>();
     // =========================== consumers (MMA + epilogue) ===========================
     const int wg = (warp - W_CONS) >> 2;                   // rows [64 wg, 64 wg + 64) of the tile
     const int wq = (warp - W_CONS) & 3;                             // warp within the warpgroup: rows 16 wq .. 16 wq + 15
@@ -439,16 +459,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_conv_umma(const ConvArgs a, con
         }
       }
       if (a.stats) {
-        // both warpgroups' sums of this 128-position tile -> global [tile128][NJ][2][Cout]; re-zero for the next tile
-        named_bar_sync(2, 256);
+        // all warpgroups' sums of this tile -> global [tile][NJ][2][Cout]; re-zero for the next tile
+        named_bar_sync(2, 32 * NCONS);
         const int et = tid - W_CONS * 32;
         unsigned long long* gp = a.stats + (size_t)(p0 / MT) * a.NJ * 2 * a.Cout;
-        for (int i = et; i < a.NJ * 2 * NT; i += 256) {
+        for (int i = et; i < a.NJ * 2 * NT; i += 32 * NCONS) {
           const int jp = i / NT, n = i - jp * NT;
           gp[(size_t)jp * a.Cout + n0 + n] = stat_s[i];
           stat_s[i] = 0ull;
         }
-        named_bar_sync(2, 256);
+        named_bar_sync(2, 32 * NCONS);
       }
     }
   }
@@ -508,9 +528,10 @@ constexpr size_t SMEM_LIMIT = 227 * 1024;
 
 size_t round1024(size_t x) { return (x + 1023) & ~(size_t)1023; }
 
-// shared-memory plan of one conv with SA slab stages (two raw stages where they fit); false when it does not fit.  Layout: slab stages, weight
-// stages, raw stages (1024-byte aligned for the swizzled TMA boxes), position table, statistics, barriers.
-bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, Plan& p) {
+// shared-memory plan of one conv with MT-position tiles and SA slab stages (two raw stages where they fit); false
+// when it does not fit.  Layout: slab stages, weight stages, raw stages (1024-byte aligned for the swizzled TMA
+// boxes), position table, statistics, barriers.
+bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, int MT, Plan& p) {
   const int Wp = ks == 3 ? W + 1 : W;
   const int Pimg = ks == 3 ? (H + 1) * (W + 1) : H * W;
   const int halo0 = ks == 3 ? Wp + 1 : 0;
@@ -576,13 +597,20 @@ int encode_map(CUtensorMap* m, const float* base, int rank, const cuuint64_t* di
   return 0;
 }
 
-template <int NT>
+template <int NT, int NWG>
 int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, cudaStream_t s) {
-  cudaError_t e = cudaFuncSetAttribute(k_conv_umma<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(k_conv_umma<NT, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   MCVD_CHECK(e == cudaSuccess, "CONV_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-  k_conv_umma<NT><<<grid, NTHREADS, smem, s>>>(a, m);
+  k_conv_umma<NT, NWG><<<grid, 128 * (NWG + 1), smem, s>>>(a, m);
   MCVD_CUDA_LAUNCH_CHECK("conv_umma");
   return 0;
+}
+
+template <int NT>
+int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, int nwg, cudaStream_t s) {
+  if constexpr (NT <= NT_MAX3)
+    if (nwg == 3) return launch_nt<NT, 3>(a, m, smem, grid, s);
+  return launch_nt<NT, 2>(a, m, smem, grid, s);
 }
 
 // common launcher: planar = the CONV_UMMA2 variant (planar norm table, K-block fixed by the caller when i2 != 0,
@@ -615,8 +643,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   a.nKB0 = (op.C0 + op.C1) / a.KB;
   a.nKB = a.nKB0 + (a.C2 + a.C3) / a.KB;
   a.tiles_n = op.Cout / NT;
-  long long tiles_m = (a.Qtot + MT - 1) / MT;
-  if (planar) tiles_m = (tiles_m + 1) & ~1LL;          // the statistics array is sized in tile pairs: write all of it
+  const long long tiles128 = (a.Qtot + STAT_MT - 1) / STAT_MT;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -632,11 +659,35 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   MCVD_CHECK(mode >= 0 && mode <= 2, "%s: work organisation %d", name, mode);
   Plan p;
   const bool can_stay = a.ks == 1 && a.nKB == a.nKB0 && a.tiles_n > 1 && a.nKB <= MAX_RESIDENT &&
-                        make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, p);
-  const bool stay = can_stay && (mode == 2 || (mode == 0 && 2 * tiles_m >= sms));
+                        make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, STAT_MT, p);
+  const bool stay = can_stay && (mode == 2 || (mode == 0 && 2 * tiles128 >= sms));
   a.SA = stay ? a.nKB : 2;
   a.NPI = stay ? a.tiles_n : 1;
-  MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, p),
+  // Tile height (CONV_UMMA i4, diagnostics): 0 = 192 positions (three consumer warpgroups) for a streaming conv
+  // without statistics whose n tile fits the accumulator registers and whose plan fits shared memory with at least
+  // three weight stages, except a 3x3 conv on maps of width >= 64 without a second segment, and unless it leaves the
+  // last SMs with more positions to cover (ceil(items / SMs) * MT): at 8x8 the 192-position items are too few to
+  // cover the SMs.  Measured on an H100 80GB HBM3 (700 W), MT = 128 -> 192: with two weight stages (64x64 at
+  // NT = 192, next to the larger slab and raw stages) the weight ring stalls the MMAs, 64x64 192->192 899 -> 1322 us;
+  // 64x64 3x3 convs without a second segment, whose slab is 1.71x the tile, 288->96 1045 -> 1135 us and 192->96
+  // 695 -> 748 us.  128 or 192 forces the height (an error where 192 cannot run).
+  const int mt_req = planar ? 0 : op.i4;
+  MCVD_CHECK(mt_req == 0 || mt_req == 128 || mt_req == 192, "%s: tile height %d", name, mt_req);
+  const bool can3 = !planar && NT <= NT_MAX3 && !stay && !a.stats &&
+                    make_plan(op.H, op.W, a.ks, a.KB, NT, false, a.SA, 192, p) &&
+                    (!a.tab || p.HP / a.Pimg + 2 <= TAB_NB);
+  MCVD_CHECK(mt_req != 192 || can3, "%s: 192-position tiles need streaming, NT <= %d, no statistics and %dx%d to fit",
+             name, NT_MAX3, op.H, op.W);
+  auto last_positions = [&](int mt) {
+    const long long items = (a.Qtot + mt - 1) / mt * a.tiles_n;
+    return (items + sms - 1) / sms * mt;
+  };
+  const bool wide_slab = a.ks == 3 && op.W >= 64 && a.nKB == a.nKB0;
+  const int MT = mt_req ? mt_req
+                        : (can3 && p.NB >= 3 && !wide_slab && last_positions(192) <= last_positions(128) ? 192 : 128);
+  long long tiles_m = (a.Qtot + MT - 1) / MT;
+  if (planar) tiles_m = (tiles_m + 1) & ~1LL;          // the statistics array is sized in tile pairs: write all of it
+  MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, MT, p),
              "%s: tile does not fit shared memory (W=%d)", name, op.W);
   a.HP = p.HP; a.NB = p.NB; a.NJ = p.NJ;
   a.boxn = p.boxn; a.nbox = p.nbox; a.raw_off = p.raw_off; a.raw_stage = p.raw_stage; a.tab_off = p.tab_off;
@@ -684,7 +735,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   a.ntiles = (int)(tiles_m * (a.tiles_n / a.NPI));
   const int grid = a.ntiles < sms ? a.ntiles : sms;
   switch (NT) {
-#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, maps, p.smem, grid, s);
+#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, maps, p.smem, grid, MT / 64, s);
     MCVD_NT_CASE(16) MCVD_NT_CASE(32) MCVD_NT_CASE(48) MCVD_NT_CASE(64) MCVD_NT_CASE(80) MCVD_NT_CASE(96)
     MCVD_NT_CASE(112) MCVD_NT_CASE(128) MCVD_NT_CASE(144) MCVD_NT_CASE(160) MCVD_NT_CASE(176) MCVD_NT_CASE(192)
     MCVD_NT_CASE(208) MCVD_NT_CASE(224) MCVD_NT_CASE(240) MCVD_NT_CASE(256)
@@ -737,7 +788,7 @@ extern "C" int mcvd_umma2_plan(int H, int W, int ks, int C0, int C1, int C2, int
   const int kb = mcvd::conv_kb(C0, C1, C2, C3);
   mcvd::Plan p;
   if (!kb || n_tile < 16 || n_tile > 256 || n_tile % 16) return 0;
-  return mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, p) ? kb : 0;
+  return mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, mcvd::STAT_MT, p) ? kb : 0;
 }
 
 // shared-memory plan of a conv (diagnostics / tests): out[0..9] = KB, HP, image stages, raw-input stages, weight
@@ -748,7 +799,7 @@ extern "C" int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2
   const int kb = mcvd_umma2_plan(H, W, ks, C0, C1, C2, C3, n_tile, stats);
   if (!kb || !out) return -1;
   mcvd::Plan p;
-  mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, p);
+  mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, mcvd::STAT_MT, p);
   out[0] = kb; out[1] = p.HP; out[2] = 2; out[3] = p.RA; out[4] = p.NB; out[5] = p.NJ; out[6] = 0;
   out[7] = (int)p.smem; out[8] = 1; out[9] = 1;
   return 0;
@@ -756,8 +807,8 @@ extern "C" int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2
 
 extern "C" long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cout) {
   const long long pimg = ks == 3 ? (long long)(H + 1) * (W + 1) : (long long)H * W;
-  const long long tiles = 2 * ((B * pimg + 2 * mcvd::MT - 1) / (2 * mcvd::MT));
-  const long long nj = (mcvd::MT - 1) / pimg + 2;
+  const long long tiles = 2 * ((B * pimg + 2 * mcvd::STAT_MT - 1) / (2 * mcvd::STAT_MT));
+  const long long nj = (mcvd::STAT_MT - 1) / pimg + 2;
   return tiles * nj * 2 * Cout * 8;
 }
 

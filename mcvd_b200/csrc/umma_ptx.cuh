@@ -61,6 +61,12 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* map, int c
       "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
       : "memory");
 }
+// per-thread register budget of the executing warpgroup, lowered (registers go back to the CTA's pool) or raised
+// (blocks until the pool holds them); every warp of the warpgroup executes it
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 

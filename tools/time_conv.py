@@ -1,8 +1,10 @@
 """Time every tensor-core conv launch of one forward of a workload (default cfg2, B = 64) with CUDA events, grouped by
 (ks, H, Cin | Csc, Cout, NT): microseconds per forward, algorithmic and executed TFLOP/s, and share of the forward.
-Algorithmic work counts 2 * pixels * Cout * (Cin * ks^2 + Csc); executed work counts every 128-position tile row
-(padding positions included) and the three fp16 products of the hi/lo split.  The GPU name and power limit are read
-(not set) in the same run.
+Algorithmic work counts 2 * pixels * Cout * (Cin * ks^2 + Csc); executed work counts every padded-flat position row
+(padding positions included) rounded up to whole 128-position tiles, and the three fp16 products of the hi/lo split.
+Convs the launcher runs in 192-position tiles execute up to 191 rather than 127 rows past the last position, which
+this count leaves out (under 0.4 % of the rows at 16x16 and above for the default batch).  The GPU name and power
+limit are read (not set) in the same run.
 
     python tools/time_conv.py [--workload cfg2] [--batch 64] [--reps 20]
 """
