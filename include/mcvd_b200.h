@@ -106,8 +106,9 @@ enum {
    * position tiles fill the GPU, else streaming; i4 = tile height, a diagnostic override of the same kind (results
    * are identical bits either way): 0 = the launcher's choice (192 positions, three consumer warpgroups, for
    * streaming convs without dst2 statistics, n tile <= 192 and at least three weight stages in shared memory, except
-   * 3x3 convs on maps of width >= 64 without a second segment and where 192 would leave SMs idle; else 128), 128 or
-   * 192 = forced (192 is an error where it cannot run); i3 = operand split for accuracy experiments (0 | 3 = all three products, 1 = drop
+   * where 192 would leave SMs idle; else 128), 128 or 192 = forced (192 is an error where it cannot run); i5 = slab
+   * stages of a streaming conv, a diagnostic override of the same kind: 0 = the launcher's choice (2), 2 or 3 =
+   * forced (an error where it does not fit or the conv is input-stationary); i3 = operand split for accuracy experiments (0 | 3 = all three products, 1 = drop
    * hi*lo_w, 2 = drop lo_a*hi, 4 = hi*hi only); f1 = weight un-scale.  Optional second K-segment (src2|src3 with C2|C3 channels, RAW,
    * centre tap only, weights appended per n-tile): the 1x1 shortcut Conv_2(x) of ResnetBlockBigGANpp
    * (layerspp.py:618-619) accumulated into the same accumulators as Conv_1, so

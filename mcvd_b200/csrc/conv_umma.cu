@@ -23,7 +23,7 @@
 // Outputs at padding positions are computed and discarded (2..20 % of the rows).
 //
 // Warp roles (128 * (NWG + 1) threads, one CTA per SM, persistent over MT x NT tiles, MT = 64 * NWG positions):
-//   warps 0-2   producers: raw fp32 NHWC stage in smem -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2 stages)
+//   warps 0-2   producers: raw fp32 NHWC stage in smem -> normalise/FiLM/SiLU -> fp16 hi/lo -> smem slab (2-3 stages)
 //               (generic-proxy stores + fence.proxy.async).  Thread 0 also issues the TMA (cp.async.bulk.tensor)
 //               loads of the raw input boxes and norm-table rows, one K-block ahead of the conversion.
 //   warp  3     weight loader: cp.async.bulk (TMA 1-D) of pre-packed fp16 hi/lo smem images (ring of NB stages)
@@ -189,9 +189,16 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
     if constexpr (NWG == 3) setmaxnreg_dec<REG_PROD3>();
     if (warp < W_LOAD) {
       // =========================== producers ===========================
-      // One thread = the slab positions h = tid + k * NPROD, all KB channels of the K-block.  The raw input and the
-      // (mean, rstd*G, S) rows of the <= tab_nb images the tile touches arrive by TMA in raw stage g % RA.
+      // One thread = one 8-channel chunk ch of the K-block over the slab positions h = h_lo + pp + k * ppass, so the
+      // norm-table row of the current image stays in its registers.  Lane l of a warp takes chunk (l / 8) % chunks
+      // and 32 / chunks consecutive positions per pass, so the eight threads of each quarter-warp read the same 16
+      // bytes of eight consecutive raw rows (distinct banks under the swizzle) and store 128 contiguous bytes.  The
+      // raw input and the (mean, rstd*G, S) rows of the <= tab_nb images the tile touches arrive by TMA in raw stage
+      // g % RA.
       const bool has_tab = a.tab != nullptr;
+      const int ch = (lane >> 3) % chunks;
+      const int ppass = NPROD / chunks;                      // positions per pass: 24 (KB = 32) or 48 (KB = 16)
+      const int pp = warp * (32 / chunks) + (lane & 7) + 8 * ((lane >> 3) / chunks);
       const uint32_t rowb = (uint32_t)a.KB * 4, smask = a.KB == 32 ? 7u : 3u;   // raw row bytes, swizzle row mask
       auto tile_b0_of = [&](int t) {
         const int q_first = (t / groups_n) * MT - a.halo0;
@@ -239,8 +246,10 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
         const int p0 = (t / groups_n) * MT;
         const int tb0 = tile_b0_of(t);
         // per tile, not per K-block: image slot << 16 | row in the first segment's raw box, or -1 for zero padding,
-        // of each position the thread owns (only this thread reads its entries)
+        // of each slab position.  Other producers read the entries (after the barrier at the top of the K-block
+        // loop), so wait until all of them are done with the previous tile's.
         const int raw_m = first_raw(a, p0 - a.halo0), raw_c = first_raw(a, p0);
+        named_bar_sync(1, NPROD);
         for (int h = tid; h < a.HP; h += NPROD) {
           int b = tb0;
           const int pix = decode_pos(a, p0 - a.halo0 + h, b);
@@ -262,56 +271,64 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
           mbar_wait(R_FULL(rs), (g / a.RA) & 1);
           const uint8_t* raw = raw_base + (size_t)rs * a.raw_stage;
           const float* tsm = reinterpret_cast<const float*>(raw + a.tab_off);
-          uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes;
+          uint8_t* hi_base = a_base + (size_t)st * a_stage_bytes + (size_t)ch * a.HP * 16;
           uint8_t* lo_base = hi_base + a_half_bytes;
-          const int h0 = h_lo + (tid - h_lo % NPROD + NPROD) % NPROD;   // first owned position >= h_lo
-#pragma unroll 1
-          for (int h = h0; h < h_hi; h += NPROD) {
-            const int info = pinfo[h];
-            const bool pad = info < 0;
-            const int bidx = info >> 16;
-            const uint32_t row = (uint32_t)((info & 0xffff) - roff);
-            float4 rv[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (j < 2 * chunks) {
-                const uint32_t off = row * rowb + 16u * j;
-                rv[j] = pad ? make_float4(0.f, 0.f, 0.f, 0.f)
-                            : *reinterpret_cast<const float4*>(raw + (off ^ (((off >> 7) & smask) << 4)));
-              }
-#pragma unroll
-            for (int ch = 0; ch < 4; ++ch) {
-              if (ch < chunks) {
-                uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
-                if (!pad) {
-                  float v[8] = {rv[2 * ch].x, rv[2 * ch].y, rv[2 * ch].z, rv[2 * ch].w,
-                                rv[2 * ch + 1].x, rv[2 * ch + 1].y, rv[2 * ch + 1].z, rv[2 * ch + 1].w};
-                  if (use_tab) {
-                    if (a.tab_planar) {                      // [tab_nb][mean | rstd*G | S][KB]
-                      const float* tb = tsm + bidx * 3 * a.KB + ch * 8;
-#pragma unroll
-                      for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tb[e], tb[a.KB + e], tb[2 * a.KB + e]);
-                    } else {                                 // [tab_nb][KB] float4 (mean, rstd, G, S)
-                      const float4* tb = reinterpret_cast<const float4*>(tsm) + bidx * a.KB + ch * 8;
-#pragma unroll
-                      for (int e = 0; e < 8; ++e) {
-                        const float4 tv = tb[e];
-                        v[e] = fmaf(v[e] - tv.x, tv.y * tv.z, tv.w);
-                      }
-                    }
-                    if (a.act_in) silu_fast8(v);
-                  }
-                  uint32_t hw[4], lw[4];
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
-                  hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                  lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                }
-                const size_t off = ((size_t)ch * a.HP + h) * 16;
-                *reinterpret_cast<uint4*>(hi_base + off) = hv;
-                *reinterpret_cast<uint4*>(lo_base + off) = lv;
-              }
+          // the 8 raw channels of chunk ch at slab position h (zeros at padding)
+          auto load_raw = [&](int info, float4& r0, float4& r1) {
+            r0 = r1 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (info >= 0) {
+              const uint32_t off = (uint32_t)((info & 0xffff) - roff) * rowb + 32u * ch;
+              const uint32_t sw = ((off >> 7) & smask) << 4;
+              r0 = *reinterpret_cast<const float4*>(raw + (off ^ sw));
+              r1 = *reinterpret_cast<const float4*>(raw + ((off + 16u) ^ sw));
             }
+          };
+          // (mean, rstd*G, S) of the cached image's 8 channels; rstd*G is the same fp32 product for every position
+          float tmean[8], tmul[8], tadd[8];
+          int tcur = -1;
+          int h = h_lo + pp;
+          int info_n = h < h_hi ? pinfo[h] : -1;
+          float4 n0, n1;
+          load_raw(info_n, n0, n1);
+#pragma unroll 1
+          for (; h < h_hi; h += ppass) {
+            const int info = info_n;
+            const float4 c0 = n0, c1 = n1;
+            // the next position's raw loads fly while this one is converted
+            info_n = h + ppass < h_hi ? pinfo[h + ppass] : -1;
+            load_raw(info_n, n0, n1);
+            uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
+            if (info >= 0) {
+              float v[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+              if (use_tab) {
+                const int bidx = info >> 16;
+                if (bidx != tcur) {
+                  tcur = bidx;
+                  if (a.tab_planar) {                        // [tab_nb][mean | rstd*G | S][KB]
+                    const float* tb = tsm + bidx * 3 * a.KB + ch * 8;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) { tmean[e] = tb[e]; tmul[e] = tb[a.KB + e]; tadd[e] = tb[2 * a.KB + e]; }
+                  } else {                                   // [tab_nb][KB] float4 (mean, rstd, G, S)
+                    const float4* tb = reinterpret_cast<const float4*>(tsm) + bidx * a.KB + ch * 8;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                      const float4 tv = tb[e];
+                      tmean[e] = tv.x; tmul[e] = tv.y * tv.z; tadd[e] = tv.w;
+                    }
+                  }
+                }
+#pragma unroll
+                for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e] - tmean[e], tmul[e], tadd[e]);
+                if (a.act_in) silu_fast8(v);
+              }
+              uint32_t hw[4], lw[4];
+#pragma unroll
+              for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
+              hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+              lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+            }
+            *reinterpret_cast<uint4*>(hi_base + (size_t)h * 16) = hv;
+            *reinterpret_cast<uint4*>(lo_base + (size_t)h * 16) = lv;
           }
           fence_proxy_async();          // make the generic-proxy stores visible to the tensor-core (async) proxy
           mbar_arrive(A_FULL(st));
@@ -661,16 +678,22 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   const bool can_stay = a.ks == 1 && a.nKB == a.nKB0 && a.tiles_n > 1 && a.nKB <= MAX_RESIDENT &&
                         make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, STAT_MT, p);
   const bool stay = can_stay && (mode == 2 || (mode == 0 && 2 * tiles128 >= sms));
-  a.SA = stay ? a.nKB : 2;
+  // Slab stages of a streaming conv (CONV_UMMA i5, diagnostics): 0 = the launcher's choice, 2 or 3 forces them.
+  const int sa_req = planar ? 0 : op.i5;
+  MCVD_CHECK(sa_req == 0 || ((sa_req == 2 || sa_req == 3) && !stay), "%s: %d slab stages", name, sa_req);
+  a.SA = stay ? a.nKB : (sa_req ? sa_req : 2);
   a.NPI = stay ? a.tiles_n : 1;
   // Tile height (CONV_UMMA i4, diagnostics): 0 = 192 positions (three consumer warpgroups) for a streaming conv
   // without statistics whose n tile fits the accumulator registers and whose plan fits shared memory with at least
-  // three weight stages, except a 3x3 conv on maps of width >= 64 without a second segment, and unless it leaves the
-  // last SMs with more positions to cover (ceil(items / SMs) * MT): at 8x8 the 192-position items are too few to
-  // cover the SMs.  Measured on an H100 80GB HBM3 (700 W), MT = 128 -> 192: with two weight stages (64x64 at
-  // NT = 192, next to the larger slab and raw stages) the weight ring stalls the MMAs, 64x64 192->192 899 -> 1322 us;
-  // 64x64 3x3 convs without a second segment, whose slab is 1.71x the tile, 288->96 1045 -> 1135 us and 192->96
-  // 695 -> 748 us.  128 or 192 forces the height (an error where 192 cannot run).
+  // three weight stages, unless it leaves the last SMs with more positions to cover (ceil(items / SMs) * MT): at 8x8
+  // the 192-position items are too few to cover the SMs.  Measured on an H100 80GB HBM3 (700 W), MT = 128 -> 192:
+  // with two weight stages (64x64 at NT = 192, next to the larger slab and raw stages) the weight ring stalls the
+  // MMAs, 64x64 192->192 827 -> 1280 us; the 64x64 3x3 convs without a second segment, whose slab is 1.71x the tile,
+  // gain from the smaller share of halo positions now that the producers keep up: 288->96 862 -> 758 us, 192->96
+  // 612 -> 521 us.  128 or 192 forces the height (an error where 192 cannot run).
+  // A third slab stage (i5 = 3) lets the producers run two K-blocks ahead, but it costs weight stages: at 64x64 it
+  // measured 192->96 608 -> 581 us at MT = 128, 521 -> 535 us at MT = 192 and 859 -> 1331 us for 192->192 at
+  // MT = 128, so the launcher keeps two.
   const int mt_req = planar ? 0 : op.i4;
   MCVD_CHECK(mt_req == 0 || mt_req == 128 || mt_req == 192, "%s: tile height %d", name, mt_req);
   const bool can3 = !planar && NT <= NT_MAX3 && !stay && !a.stats &&
@@ -682,9 +705,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
     const long long items = (a.Qtot + mt - 1) / mt * a.tiles_n;
     return (items + sms - 1) / sms * mt;
   };
-  const bool wide_slab = a.ks == 3 && op.W >= 64 && a.nKB == a.nKB0;
-  const int MT = mt_req ? mt_req
-                        : (can3 && p.NB >= 3 && !wide_slab && last_positions(192) <= last_positions(128) ? 192 : 128);
+  const int MT = mt_req ? mt_req : (can3 && p.NB >= 3 && last_positions(192) <= last_positions(128) ? 192 : 128);
   long long tiles_m = (a.Qtot + MT - 1) / MT;
   if (planar) tiles_m = (tiles_m + 1) & ~1LL;          // the statistics array is sized in tile pairs: write all of it
   MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, MT, p),
