@@ -138,7 +138,9 @@ enum {
    *   i3   = operand split: 3 (default, also 0) = hi*hi + lo*hi + hi*lo, 1 = drop hi*lo (fp16 weights),
    *          2 = drop lo*hi (fp16 activations), 4 = hi*hi only -- accuracy experiments;
    *   dst2 = NULL, or int64 [tiles][NJ][2][Cout] receiving the GroupNorm partial sums of the stored output
-   *          (sum and sum of squares of round(x * 2^16), exact integer arithmetic; tiles = 128-position row
+   *          (sum and sum of squares of round(x * 2^16), exact integer arithmetic for |x| <= 2^12: round(x * 2^16)
+   *          stays inside int32 and the sum of squares of a tile slot's 128 rows inside 64 bits; outputs beyond
+   *          that range have no defined statistics; tiles = 128-position row
    *          tiles of the padded-flat position space, NJ = 127 / Pimg + 2 image slots per tile,
    *          mcvd_umma2_stats_bytes() bytes) -- nn.GroupNorm statistics of the NEXT act-norm
    *          (layerspp.py:474-477) without re-reading the activation;

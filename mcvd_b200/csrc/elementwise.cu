@@ -255,17 +255,19 @@ __global__ void __launch_bounds__(128) k_gn_partial(const float* __restrict__ s0
     const float* ptr = src + ((long long)b * HW + p0) * cs + cc;
     double ds = 0.0, dq = 0.0;
     int p = p0;
-    // 8 independent loads in flight per lane; fp32 partials over 8 pixels, fp64 across groups
+    // 8 independent loads in flight per lane, every sum in fp64: fp32 partials would cost the variance
+    // E[x^2] - mean^2 all its bits once |mean| >> std
     for (; p + 8 <= p1; p += 8) {
       float v[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = __ldg(ptr + (long long)i * cs);
       ptr += 8LL * cs;
-      float fs = 0.f, fq = 0.f;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) { fs += v[i]; fq = fmaf(v[i], v[i], fq); }
-      ds += (double)fs;
-      dq += (double)fq;
+      for (int i = 0; i < 8; ++i) {
+        const double d = (double)v[i];
+        ds += d;
+        dq = fma(d, d, dq);
+      }
     }
     for (; p < p1; ++p) {
       const float v = __ldg(ptr);

@@ -10,6 +10,7 @@ import torch.nn.functional as F
 
 from mcvd_b200 import lib
 from mcvd_b200.lib import McvdOp
+from op_interpreter import tile_stats
 
 pytestmark = pytest.mark.gpu
 
@@ -67,22 +68,9 @@ def pack2(t_main, t_sc, nt, kb):
 
 
 def expected_stats(y, ks):
-    """what the epilogue must have written for the stored output y [B,H,W,C] (tests/op_interpreter.py semantics)"""
-    B, H, W, C = y.shape
-    pimg = (H + 1) * (W + 1) if ks == 3 else H * W
-    nj, ntiles = 127 // pimg + 2, 2 * ((B * pimg + 255) // 256)
-    st = torch.zeros(ntiles, nj, 2, C, dtype=torch.int64)
-    xi = torch.round(y.double() * 65536.0).clamp(-(1 << 28), 1 << 28).to(torch.int64)
-    yy, xx = torch.meshgrid(torch.arange(H), torch.arange(W), indexing="ij")
-    r = ((yy + 1) * (W + 1) + xx + 1) if ks == 3 else (yy * W + xx)
-    for b in range(B):
-        q = (b * pimg + r).reshape(-1)
-        t = q // 128
-        jj = b - torch.clamp((t * 128) // pimg, max=B - 1)
-        v = xi[b].reshape(H * W, C)
-        st[:, :, 0].index_put_((t, jj), v, accumulate=True)
-        st[:, :, 1].index_put_((t, jj), v * v, accumulate=True)
-    return st
+    """what the epilogue must have written for the stored output y [B,H,W,C] (tests/op_interpreter.py semantics;
+    raises ValueError outside the statistics' range |y| <= 2^12)"""
+    return tile_stats(y, ks)
 
 
 CASES = [

@@ -175,6 +175,18 @@ def test_groupnorm_table(B, H, C0, C1):
         assert torch.equal(tab2, tab)
 
 
+def test_groupnorm_partials_are_float64():
+    """|mean| >> std: the variance E[x^2] - mean^2 keeps its bits only if every partial sum is fp64 (sums of 8 pixels
+    in fp32 were 2^-24 relative, which cost rstd its leading digits here)"""
+    B, H, C, nchunk = 2, 16, 32, 4
+    x = 300.0 + rnd(B, H, H, C, seed=4) * 0.01
+    part = torch.zeros(B * nchunk * C * 2, dtype=torch.float64, device=DEV)
+    run([mk(lib.OP_GN_PARTIAL, B, H=H, W=H, C0=C, i0=nchunk, src0=x.to(DEV).contiguous(), dst=part)])
+    xd = x.double().view(B, nchunk, H * H // nchunk, C)
+    ref = torch.stack([xd.sum(2), (xd * xd).sum(2)], 3).reshape(-1)
+    assert ((part.cpu() - ref).abs() <= 1e-12 * ref).all()
+
+
 @pytest.mark.parametrize("mode", ["none", "down", "up"])
 @pytest.mark.parametrize("spade", [False, True])
 @pytest.mark.parametrize("B,Hin,C0,C1", [(2, 16, 32, 16),     # 48 channels: a full and a half 32-channel chunk
