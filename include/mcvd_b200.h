@@ -202,6 +202,21 @@ enum {
    * with bias (w = fp32 [C0][Cout], bias fp32 [Cout]), mean over time.  src0 [B, i4, 7, 7, C0] (i5 = 7, i4 >= 2),
    * dst fp64 [B, Cout] (Cout <= 512, C0 <= 6144); all in fp64, fixed reduction order, no atomics.  H = W = 1. */
   MCVD_OP_I3D_HEAD = 25,
+  /* Perturbation of the denoising score-matching loss (losses/dsm.py:anneal_dsm_score_estimation, DDPM branch):
+   * src0 = clean frames x [B, C0, H, W] fp32 NCHW (data-transformed); aux0 = fp32 table [B][4] per clip:
+   * sqrt(a_b), sqrt(1 - a_b), Gamma shape k_b (finite, > 0), Gamma scale s_b.  dst = x_t = sqrt(a_b) x + sqrt(1 - a_b) z,
+   * evaluated as two rounded fp32 products and one rounded add (no FMA contraction), as torch evaluates the reference's
+   * expression.  MCVD_F_PHILOX: z is the Philox normal keyed as in MCVD_OP_DIFFUSION_UPDATE (seed i0|i1<<32, clip id
+   * i2 + b, step tag i3, element c*H*W + p) and is written to dst2; with MCVD_F_GAMMA as well z = s_b * (G - k_b),
+   * G ~ Gamma(k_b, 1) drawn in-kernel with the shape of each clip's row.  Without MCVD_F_PHILOX z is read from src1
+   * (injected noise; dst2 = NULL or a copy of it). */
+  MCVD_OP_DSM_PERTURB = 26,
+  /* Per-clip loss of the denoising score-matching objective: src0 = eps [B, H, W, C0] NHWC (channel pitch Cout if
+   * > 0, the network output as MCVD_OP_DIFFUSION_UPDATE reads it), src1 = z [B, C0, H, W] NCHW; dst = fp64 [B],
+   * dst[b] = sum over the clip of 0.5 (z - eps)^2, or of |z - eps| with MCVD_F_L1.  The difference is rounded to fp32
+   * (as in the reference) and summed in fp64; one CTA per clip with a fixed reduction order and no atomics, so a
+   * clip's value is the same bits at any batch size and batch position. */
+  MCVD_OP_DSM_LOSS = 27,
   MCVD_OP__COUNT
 };
 
@@ -212,10 +227,12 @@ enum {
 #define MCVD_F_DOWN     (1 << 3)   /* APPLY: FIR downsample x2 (input is 2H x 2W)                 */
 #define MCVD_F_FILM     (1 << 4)   /* GN_FINALIZE: aux0 is the FiLM table                          */
 #define MCVD_F_CLIP     (1 << 5)   /* DIFFUSION_UPDATE: clamp x0 to [-1, 1]                        */
-#define MCVD_F_PHILOX   (1 << 6)   /* DIFFUSION_UPDATE: draw z in-kernel                           */
+#define MCVD_F_PHILOX   (1 << 6)   /* DIFFUSION_UPDATE, DSM_PERTURB: draw z in-kernel              */
 #define MCVD_F_ROUND    (1 << 7)   /* FRAME_METRICS: round the images before the grey conversion   */
-#define MCVD_F_GAMMA    (1 << 8)   /* DIFFUSION_UPDATE (with PHILOX), NOISE: centred Gamma(f6) * f7 */
+#define MCVD_F_GAMMA    (1 << 8)   /* DIFFUSION_UPDATE (with PHILOX), NOISE: centred Gamma(f6) * f7;
+                                      DSM_PERTURB (with PHILOX): per-clip shape and scale from aux0 */
 #define MCVD_F_POOL     (1 << 9)   /* CONV_RELU: 3x3 / stride-2 max-pool on the input read           */
+#define MCVD_F_L1       (1 << 10)  /* DSM_LOSS: sum |z - eps| instead of 0.5 (z - eps)^2               */
 
 typedef struct McvdOp {
   int32_t kind;

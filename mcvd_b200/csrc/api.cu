@@ -42,6 +42,8 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_CONV3D: return launch_conv3d(op, s);
     case MCVD_OP_MAXPOOL3D: return launch_maxpool3d(op, s);
     case MCVD_OP_I3D_HEAD: return launch_i3d_head(op, s);
+    case MCVD_OP_DSM_PERTURB: return launch_dsm_perturb(op, s);
+    case MCVD_OP_DSM_LOSS: return launch_dsm_loss(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -168,6 +170,13 @@ static int validate_one(const McvdOp& op, int idx) {
       }
       break;
     }
+    case MCVD_OP_DSM_PERTURB:
+    case MCVD_OP_DSM_LOSS:
+      if (const char* why = dsm_error(op)) {
+        set_error("op %d %s: %s", idx, op.kind == MCVD_OP_DSM_PERTURB ? "DSM_PERTURB" : "DSM_LOSS", why);
+        return -1;
+      }
+      break;
     default: break;
   }
   return 0;

@@ -37,6 +37,8 @@ OP_I3D_PREP = 22
 OP_CONV3D = 23
 OP_MAXPOOL3D = 24
 OP_I3D_HEAD = 25
+OP_DSM_PERTURB = 26
+OP_DSM_LOSS = 27
 
 F_ACT_IN = 1 << 0
 F_ACT_OUT = 1 << 1
@@ -48,6 +50,7 @@ F_PHILOX = 1 << 6
 F_ROUND = 1 << 7
 F_GAMMA = 1 << 8
 F_POOL = 1 << 9
+F_L1 = 1 << 10
 
 ABI_VERSION = 5
 

@@ -1,4 +1,4 @@
-"""Drop-in shim: make the UNMODIFIED reference (``main.py --config ... --video_gen``,
+"""Drop-in shim: make the UNMODIFIED reference (``main.py --config ... --video_gen`` and ``--test``,
 ``load_model_from_ckpt.py``, the demo notebook) use the H100 path.
 
     import mcvd_b200.patch; mcvd_b200.patch.install()      # before NCSNRunner / load_model are used
@@ -12,6 +12,11 @@ cover (3-D archs, ``noise_in_cond``, ``cond_emb``, ``output_all_frames``, SMLD, 
 reference implementation: same results, no acceleration.  ``torch.nn.DataParallel`` wrappers are
 accepted (the samplers unwrap ``.module``), but multi-GPU runs should use ``runner.video_gen_sharded``
 (one process per GPU) instead of DataParallel's per-call weight broadcast.
+
+The test loss ``losses.dsm.anneal_dsm_score_estimation`` (and the name ``runners.ncsn_runner`` imported) is
+rebound too: a native network evaluated with grad mode off and without ``all_frames`` (``NCSNRunner.test``) gets the
+native loss (``mcvd_b200.dsm``), whose noise is drawn in-kernel; every other call -- reference models, training, which
+needs gradients -- keeps the reference function.
 """
 from __future__ import annotations
 
@@ -54,6 +59,26 @@ def install(verbose: bool = True):
         return sampler
 
     R.get_model = get_model
+    try:
+        import losses.dsm as LD
+    except ImportError:                           # a tree without the training code: nothing to rebind
+        LD = None
+    if LD is not None:
+        from . import dsm as fast_dsm
+        ref_dsm = LD.anneal_dsm_score_estimation
+
+        @functools.wraps(ref_dsm)
+        def anneal_dsm_score_estimation(scorenet, *a, **kw):
+            net = scorenet.module if hasattr(scorenet, "module") else scorenet
+            # all_frames is the reference signature's 10th parameter: (scorenet, x, labels, loss_type, hook, cond,
+            # cond_mask, gamma, L1, all_frames)
+            all_frames = kw.get("all_frames", a[8] if len(a) > 8 else False)
+            if isinstance(net, fast_model.UNetMore_DDPM) and not torch.is_grad_enabled() and not all_frames:
+                return fast_dsm.anneal_dsm_score_estimation(scorenet, *a, **kw)
+            return ref_dsm(scorenet, *a, **kw)
+        LD.anneal_dsm_score_estimation = anneal_dsm_score_estimation
+        if hasattr(R, "anneal_dsm_score_estimation"):
+            R.anneal_dsm_score_estimation = anneal_dsm_score_estimation
     for name in ref_samplers:
         fn = dispatch(name)
         setattr(M, name, fn)

@@ -19,6 +19,7 @@ from __future__ import annotations
 import contextlib
 import math
 import os
+import types
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -131,6 +132,7 @@ class Engine:
         self.packs_loaded = 0
         self.programs: Dict[int, Program] = {}
         self.launches_last_forward = 0
+        self.launches_last_dsm = 0
 
     # ------------------------------------------------------------------------------ weights
     MAX_PROGRAMS = 3                 # lowered programs (one per batch size) kept alive; least recently used goes first
@@ -804,3 +806,80 @@ class Engine:
             self._run(P.out_arr, 1)
             self.launches_last_forward = P.cond_launches + P.step_launches + 1
             return P.out.clone()
+
+    # ------------------------------------------------------------------------------ denoising score matching
+    def _dsm_buffers(self, P: Program):
+        """Clean frames, noise, per-clip coefficient table, fp64 per-clip loss and the two ops around the network,
+        allocated on a program's first DSM call."""
+        if getattr(P, "dsm", None) is not None:
+            return P.dsm
+        ns, B, S = self.spec, P.B, self.spec.image_size
+        D = types.SimpleNamespace()
+        D.x = torch.empty(B, ns.out_ch, S, S, device=self.device, dtype=torch.float32)
+        D.z = torch.empty_like(D.x)
+        D.tab = torch.zeros(B, 4, device=self.device, dtype=torch.float32)
+        D.loss = torch.empty(B, device=self.device, dtype=torch.float64)
+        if self.backend is not None:
+            for t in (D.x, D.z, D.tab, D.loss):
+                self.backend.register(t)
+        p = McvdOp()
+        p.kind, p.B, p.H, p.W, p.C0 = lib.OP_DSM_PERTURB, B, S, S, ns.out_ch
+        p.src0, p.src1, p.aux0, p.dst = D.x.data_ptr(), D.z.data_ptr(), D.tab.data_ptr(), P.x_in.data_ptr()
+        D.perturb_arr = lib.make_ops([p])
+        o = McvdOp()
+        o.kind, o.B, o.H, o.W, o.C0, o.Cout = lib.OP_DSM_LOSS, B, S, S, ns.out_ch, P.eps_nhwc.shape[-1]
+        o.src0, o.src1, o.dst = P.eps_nhwc.data_ptr(), D.z.data_ptr(), D.loss.data_ptr()
+        D.loss_arr = lib.make_ops([o])
+        lib.validate_program(D.perturb_arr, 1)
+        lib.validate_program(D.loss_arr, 1)
+        P.dsm = D
+        return D
+
+    def dsm(self, x, labels, cond=None, *, z=None, philox=None, gamma=False, l1=False):
+        """Per-clip denoising score-matching loss (reference losses/dsm.py, DDPM branch) as a float64 [B] tensor.
+
+        ``x`` [B, C*F, S, S] are the clean, data-transformed frames, ``labels`` [B] the noise levels.  The noise is
+        either injected (``z``: the reference's standardised noise) or drawn in-kernel (``philox = (seed, clip0,
+        step tag)``: the Philox stream of clip ``clip0 + b``), Gamma-distributed with ``gamma``.  Runs the
+        perturbation into the network input, the cond ops, the network with per-clip timesteps and the loss: the
+        network's launches plus 2.  Afterwards the program's ``x_in`` holds x_t and ``dsm.z`` the noise."""
+        ns = self.spec
+        B = x.shape[0]
+        if ns.cond_ch > 0 and cond is None:
+            raise RuntimeError("mcvd_b200: this network was built with conditioning frames; cond is required")
+        if (z is None) == (philox is None):
+            raise ValueError("mcvd_b200 dsm: pass exactly one of z (injected noise) and philox (in-kernel draw)")
+        if gamma and philox is not None and not getattr(self.module, "gamma", False):
+            raise ValueError("mcvd_b200 dsm: Gamma noise needs a model built with model.gamma=True (k_cum, theta_t)")
+        with self._devctx():
+            P = self.program(B)
+            D = self._dsm_buffers(P)
+            D.x.copy_(x.reshape(D.x.shape))
+            lab = labels.to(self.device).long().reshape(-1)
+            alphas = self.module.alphas
+            used = alphas[lab]
+            # the reference's fp32 expressions (losses/dsm.py): used_alphas.sqrt(), (1 - used_alphas).sqrt(), and for
+            # Gamma noise the shape k_cum and the scale theta_t / sqrt(1 - a) of z = (G theta - k theta) / sqrt(1 - a)
+            D.tab[:, 0] = used.sqrt()
+            D.tab[:, 1] = (1 - used).sqrt()
+            op = D.perturb_arr[0]
+            if philox is not None:
+                seed, clip0, step = (int(v) for v in philox)
+                op.flags = lib.F_PHILOX
+                op.i0, op.i1, op.i2, op.i3 = seed & 0x7FFFFFFF, (seed >> 31) & 0x7FFFFFFF, clip0, step
+                op.dst2 = D.z.data_ptr()
+                if gamma:
+                    op.flags |= lib.F_GAMMA
+                    D.tab[:, 2] = self.module.k_cum[lab]
+                    D.tab[:, 3] = self.module.theta_t[lab] / (1 - used).sqrt()
+            else:
+                D.z.copy_(z.reshape(D.z.shape))
+                op.flags, op.dst2 = 0, None
+            D.loss_arr[0].flags = lib.F_L1 if l1 else 0
+            self.set_inputs(P, t=lab, cond=None if cond is None else cond.float())
+            self._run(D.perturb_arr, 1)
+            self.run_cond(P)
+            self.run_step(P)
+            self._run(D.loss_arr, 1)
+            self.launches_last_dsm = P.cond_launches + P.step_launches + 2
+            return D.loss.clone()

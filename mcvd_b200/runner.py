@@ -464,3 +464,48 @@ def evaluate_clips(config, scorenet, X: torch.Tensor, preds_per_test: Optional[i
     task = "interp" if getattr(config.data, "num_frames_future", 0) > 0 else "pred"
     return evaluate_tasks(config, scorenet, X, preds_per_test, tasks=[task], num_frames_pred=num_frames_pred,
                           lpips=lpips, i3d=i3d, **gen_kw)[task]
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the reference's test loss (main.py --test)
+# ---------------------------------------------------------------------------------------------------------------
+@torch.no_grad()
+def test_loss(config, scorenet, X: torch.Tensor, labels: Optional[torch.Tensor] = None,
+              philox_seed: Optional[int] = None, clip_offset: int = 0) -> Dict[str, torch.Tensor]:
+    """Denoising score-matching loss of one test batch, as ``NCSNRunner.test`` scores it (runners/ncsn_runner.py:
+    2402-2418): ``data_transform``, then ``conditioning_fn`` with the training masks ``data.prob_mask_cond`` /
+    ``data.prob_mask_future`` (drawn from torch's generator, as the reference does), then the loss with ``model.gamma``
+    and ``training.L1`` from the config (``mcvd_b200.dsm``).
+
+    ``X`` is [B, T, C, S, S] in [0, 1].  ``labels`` default to ``randint(0, num levels)``; the noise of global clip
+    ``clip_offset + b`` is drawn from ``philox_seed`` (from torch's default generator when None), so with fixed labels
+    and seed a batch split into shards gives the same bits per clip.  Returns ``{"loss": per-clip float64 [B],
+    "labels": [B], "mean": float64 scalar}``; the reference logs ``mean``."""
+    from . import dsm
+    from .model import UNetMore_DDPM
+    net = scorenet.module if hasattr(scorenet, "module") else scorenet
+    if not isinstance(net, UNetMore_DDPM):
+        raise TypeError(f"mcvd_b200.runner.test_loss drives mcvd_b200.UNetMore_DDPM modules (got {type(net).__name__})")
+    dev = next(net.parameters()).device
+    X = data_transform(config, X.to(dev))
+    x, cond, _ = conditioning_fn(config, X, num_frames_pred=config.data.num_frames,
+                                 prob_mask_cond=getattr(config.data, "prob_mask_cond", 0.0),
+                                 prob_mask_future=getattr(config.data, "prob_mask_future", 0.0),
+                                 conditional=config.data.num_frames_cond > 0)
+    if labels is None:
+        labels = torch.randint(0, len(net.alphas), (x.shape[0],), device=dev)
+    if philox_seed is None:
+        philox_seed = samplers.draw_seed()
+    l1 = getattr(getattr(config, "training", None), "L1", False)
+    loss = net.engine().dsm(x, labels, cond, philox=(philox_seed, clip_offset, dsm.DSM_STEP),
+                            gamma=getattr(config.model, "gamma", False), l1=l1)
+    return {"loss": loss, "labels": labels, "mean": loss.mean()}
+
+
+def loss_per_level(loss: torch.Tensor, labels: torch.Tensor, num_classes: int) -> torch.Tensor:
+    """Mean loss per noise level, float64 [num_classes], NaN where no clip has that level: the breakdown of the
+    reference's ``test_hook`` (runners/ncsn_runner.py:317-320), with one scatter of (loss, 1) pairs."""
+    pairs = torch.stack([loss.double(), torch.ones_like(loss, dtype=torch.float64)], dim=1)
+    acc = torch.zeros(num_classes, 2, dtype=torch.float64, device=loss.device)
+    acc.index_add_(0, labels.to(loss.device).long(), pairs)
+    return acc[:, 0] / acc[:, 1]
