@@ -217,6 +217,42 @@ enum {
    * (as in the reference) and summed in fp64; one CTA per clip with a fixed reduction order and no atomics, so a
    * clip's value is the same bits at any batch size and batch position. */
   MCVD_OP_DSM_LOSS = 27,
+  /* FID input of frames (evaluation/inception.py:146-153, InceptionV3.forward with resize_input and
+   * normalize_input): src0 = frames [B, C0, i1, i1] fp32 (C0 = 1|3, side i1), bilinear resize to 299x299
+   * (F.interpolate align_corners=False: src = (dst + 0.5) * i1 / 299 - 0.5, clamped at 0; no antialias), then
+   * 2x - 1, no clamp, no quantisation; a grey frame is replicated to RGB (the reference raises on it).
+   * dst = fp32 NHWC [B, 299, 299, 4], channel 3 zero.  H = W = 299; B <= 65535. */
+  MCVD_OP_FID_PREP = 28,
+  /* NHWC 2-D convolution + bias + ReLU (fp32 FFMA implicit GEMM): one BasicConv2d of torchvision's Inception3
+   * (conv without bias, BatchNorm2d(eps=0.001) folded into w and bias on the host, ReLU).  src0 [B, i5, i5, C0]
+   * (C0 a multiple of 4); kernel i0 x i1 (rows x columns), stride i2, zero padding i3 rows and i4 columns per side;
+   * output H = (i5 + 2 i3 - i0) / i2 + 1, W = (i5 + 2 i4 - i1) / i2 + 1.  w = fp32 [i0][i1][C0][Cout] (K-major),
+   * bias [Cout], Cout a multiple of 8.  The output is channels [i7, i7 + Cout) of dst [B, H, W, i6] (i6 = channel
+   * pitch >= i7 + Cout, both multiples of 4); other channels are not written, so an Inception block's branches
+   * write their torch.cat in place.  MCVD_F_POOL (1x1 stride-1 kernels only): the conv reads the 3x3 / stride-1 /
+   * pad-1 pool of src0 -- max, where padding never wins (FIDInceptionE_2, evaluation/inception.py:320-325), or with
+   * MCVD_F_AVG the average with count_include_pad=False (FIDInceptionA/C/E_1, :226-230, 254-258, 287-291).  Each
+   * output is accumulated by one thread in K order. */
+  MCVD_OP_CONV2D = 29,
+  /* nn.MaxPool2d(kernel_size=3, stride=2) without padding (evaluation/inception.py:91, 101; the pool branches of
+   * torchvision's InceptionB and InceptionD): src0 [B, i5, i5, C0] (C0 a multiple of 4), H = W = (i5 - 3) / 2 + 1;
+   * the output is channels [i7, i7 + C0) of dst [B, H, W, i6] (pitch and offset as for CONV2D). */
+  MCVD_OP_MAXPOOL2D = 30,
+  /* AdaptiveAvgPool2d(1) of the last Inception map (evaluation/inception.py:118): src0 [B, i5, i5, C0] fp32,
+   * dst fp64 [B, C0], the mean over the i5 * i5 positions summed in raster order in fp64, no atomics.  H = W = 1. */
+  MCVD_OP_FID_HEAD = 31,
+  /* k-NN radius of precision / recall (evaluation/fid_PR.py:252-253, calc_cdist_full(...).kthvalue(k+1)):
+   * src0 = A fp32 [B, C0], src1 = the second set fp32 [i0, C0] (C0 a multiple of 4); dst fp32 [B]: for every row a
+   * the i1-th smallest (1 <= i1 <= 8, i1 <= i0) of d(a, b) over the rows b of src1, duplicates counted as
+   * torch.kthvalue counts them (with A = src1, a's distance to itself, exactly 0, is one of them).  d(a, b) = sqrtf
+   * of the fp32 sum over features 0 .. C0-1, in that order, of (a - b)^2 -- not cdist's |a|^2 + |b|^2 - 2ab.  No
+   * distance matrix is stored: O(B) state.  H = W = 1. */
+  MCVD_OP_KNN_RADIUS = 32,
+  /* k-NN cover of precision / recall (evaluation/fid_PR.py:256-259): src0 = A [B, C0], src1 = the second set
+   * [i0, C0], aux0 = its radii fp32 [i0] (MCVD_OP_KNN_RADIUS of src1 over itself); dst int32 [B] = 1 if some row b
+   * has d(a, b) <= aux0[b], else 0, with the distance of MCVD_OP_KNN_RADIUS.  Precision is the mean of the flags of
+   * the fake set over the real one, recall the converse.  H = W = 1. */
+  MCVD_OP_KNN_COVER = 33,
   MCVD_OP__COUNT
 };
 
@@ -231,8 +267,10 @@ enum {
 #define MCVD_F_ROUND    (1 << 7)   /* FRAME_METRICS: round the images before the grey conversion   */
 #define MCVD_F_GAMMA    (1 << 8)   /* DIFFUSION_UPDATE (with PHILOX), NOISE: centred Gamma(f6) * f7;
                                       DSM_PERTURB (with PHILOX): per-clip shape and scale from aux0 */
-#define MCVD_F_POOL     (1 << 9)   /* CONV_RELU: 3x3 / stride-2 max-pool on the input read           */
+#define MCVD_F_POOL     (1 << 9)   /* CONV_RELU: 3x3 / stride-2 max-pool on the input read;
+                                      CONV2D: 3x3 / stride-1 / pad-1 max-pool on the input read     */
 #define MCVD_F_L1       (1 << 10)  /* DSM_LOSS: sum |z - eps| instead of 0.5 (z - eps)^2               */
+#define MCVD_F_AVG      (1 << 11)  /* CONV2D (with POOL): average pool, count_include_pad=False        */
 
 typedef struct McvdOp {
   int32_t kind;

@@ -44,6 +44,12 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_I3D_HEAD: return launch_i3d_head(op, s);
     case MCVD_OP_DSM_PERTURB: return launch_dsm_perturb(op, s);
     case MCVD_OP_DSM_LOSS: return launch_dsm_loss(op, s);
+    case MCVD_OP_FID_PREP: return launch_fid_prep(op, s);
+    case MCVD_OP_CONV2D: return launch_conv2d(op, s);
+    case MCVD_OP_MAXPOOL2D: return launch_maxpool2d(op, s);
+    case MCVD_OP_FID_HEAD: return launch_fid_head(op, s);
+    case MCVD_OP_KNN_RADIUS:
+    case MCVD_OP_KNN_COVER: return launch_knn(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -177,6 +183,28 @@ static int validate_one(const McvdOp& op, int idx) {
         return -1;
       }
       break;
+    case MCVD_OP_FID_PREP:
+    case MCVD_OP_CONV2D:
+    case MCVD_OP_MAXPOOL2D:
+    case MCVD_OP_FID_HEAD:
+    case MCVD_OP_KNN_RADIUS:
+    case MCVD_OP_KNN_COVER: {
+      const char* why = op.kind == MCVD_OP_FID_PREP    ? fid_prep_error(op)
+                        : op.kind == MCVD_OP_CONV2D    ? conv2d_error(op)
+                        : op.kind == MCVD_OP_MAXPOOL2D ? maxpool2d_error(op)
+                        : op.kind == MCVD_OP_FID_HEAD  ? fid_head_error(op)
+                                                       : knn_error(op);
+      static const char* const names[] = {"FID_PREP", "CONV2D", "MAXPOOL2D", "FID_HEAD", "KNN_RADIUS", "KNN_COVER"};
+      if (why) {
+        set_error("op %d %s: %s", idx, names[op.kind - MCVD_OP_FID_PREP], why);
+        return -1;
+      }
+      if (misaligned(op.bias)) {
+        set_error("op %d %s: bias must be 16-byte aligned", idx, names[op.kind - MCVD_OP_FID_PREP]);
+        return -1;
+      }
+      break;
+    }
     default: break;
   }
   return 0;

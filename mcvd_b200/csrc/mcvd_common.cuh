@@ -60,6 +60,11 @@ int launch_maxpool3d(const McvdOp& op, cudaStream_t s);
 int launch_i3d_head(const McvdOp& op, cudaStream_t s);
 int launch_dsm_perturb(const McvdOp& op, cudaStream_t s);
 int launch_dsm_loss(const McvdOp& op, cudaStream_t s);
+int launch_fid_prep(const McvdOp& op, cudaStream_t s);
+int launch_conv2d(const McvdOp& op, cudaStream_t s);
+int launch_maxpool2d(const McvdOp& op, cudaStream_t s);
+int launch_fid_head(const McvdOp& op, cudaStream_t s);
+int launch_knn(const McvdOp& op, cudaStream_t s);
 
 // NULL, or why the geometry of a MCVD_OP_CONV_RELU op is unusable
 const char* conv_relu_error(const McvdOp& op);
@@ -72,6 +77,13 @@ const char* i3d_head_error(const McvdOp& op);
 
 // NULL, or why a MCVD_OP_DSM_PERTURB / MCVD_OP_DSM_LOSS op is unusable (shared by validation and launch; dsm.cu)
 const char* dsm_error(const McvdOp& op);
+
+// NULL, or why an op of the FID kinds is unusable (shared by validation and launch; inception.cu, knn.cu)
+const char* fid_prep_error(const McvdOp& op);
+const char* conv2d_error(const McvdOp& op);
+const char* maxpool2d_error(const McvdOp& op);
+const char* fid_head_error(const McvdOp& op);
+const char* knn_error(const McvdOp& op);
 
 // NULL, or why the Gamma parameters (f6 = shape, f7 = scale) of an op with MCVD_F_GAMMA are unusable
 const char* gamma_params_error(const McvdOp& op);

@@ -39,6 +39,12 @@ OP_MAXPOOL3D = 24
 OP_I3D_HEAD = 25
 OP_DSM_PERTURB = 26
 OP_DSM_LOSS = 27
+OP_FID_PREP = 28
+OP_CONV2D = 29
+OP_MAXPOOL2D = 30
+OP_FID_HEAD = 31
+OP_KNN_RADIUS = 32
+OP_KNN_COVER = 33
 
 F_ACT_IN = 1 << 0
 F_ACT_OUT = 1 << 1
@@ -51,6 +57,7 @@ F_ROUND = 1 << 7
 F_GAMMA = 1 << 8
 F_POOL = 1 << 9
 F_L1 = 1 << 10
+F_AVG = 1 << 11
 
 ABI_VERSION = 5
 

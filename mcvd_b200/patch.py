@@ -17,6 +17,13 @@ The test loss ``losses.dsm.anneal_dsm_score_estimation`` (and the name ``runners
 rebound too: a native network evaluated with grad mode off and without ``all_frames`` (``NCSNRunner.test``) gets the
 native loss (``mcvd_b200.dsm``), whose noise is drawn in-kernel; every other call -- reference models, training, which
 needs gradients -- keeps the reference function.
+
+``evaluation.fid_PR.get_fid``, ``get_fid_PR`` and ``get_PR`` (and the names ``runners.ncsn_runner`` imported, used by
+``--fast_fid`` and ``--sample`` with ``sampling.fid``) are rebound to ``mcvd_b200.fid``: Inception features and
+k-NN precision / recall on the GPU, without the N x N host matrices.  The native version runs when the FID weights
+(``pt_inception-2015-12-05-6726825d.pth``) are in the torch hub cache (``torch.hub.get_dir()/checkpoints``, where
+the reference's download puts them), ``dims == 2048`` and the device is CUDA; otherwise the reference function runs.
+The native path never downloads.
 """
 from __future__ import annotations
 
@@ -79,6 +86,33 @@ def install(verbose: bool = True):
         LD.anneal_dsm_score_estimation = anneal_dsm_score_estimation
         if hasattr(R, "anneal_dsm_score_estimation"):
             R.anneal_dsm_score_estimation = anneal_dsm_score_estimation
+    try:
+        import evaluation.fid_PR as EF
+    except ImportError:                           # a tree without the evaluation code: nothing to rebind
+        EF = None
+    if EF is not None:
+        from . import fid as fast_fid
+
+        def fid_dispatch(name):
+            ref_fn, fast_fn = getattr(EF, name), getattr(fast_fid, name)
+
+            @functools.wraps(ref_fn)
+            def fn(*a, **kw):
+                # (real | path1, fake | path2, device, batch_size, dims, ...) in all three signatures
+                device = kw.get("device", a[2] if len(a) > 2 else "cuda")
+                dims = kw.get("dims", a[4] if len(a) > 4 else 2048)
+                why = fast_fid.native_unsupported(device, dims)
+                if why is None:
+                    return fast_fn(*a, **kw)
+                if verbose:
+                    print(f"[mcvd_b200] {name}: falling back to the reference: {why}", file=sys.stderr)
+                return ref_fn(*a, **kw)
+            return fn
+        for name in ("get_fid", "get_fid_PR", "get_PR"):
+            fn = fid_dispatch(name)
+            setattr(EF, name, fn)
+            if hasattr(R, name):
+                setattr(R, name, fn)
     for name in ref_samplers:
         fn = dispatch(name)
         setattr(M, name, fn)
