@@ -253,6 +253,19 @@ enum {
    * has d(a, b) <= aux0[b], else 0, with the distance of MCVD_OP_KNN_RADIUS.  Precision is the mean of the flags of
    * the fake set over the real one, recall the converse.  H = W = 1. */
   MCVD_OP_KNN_COVER = 33,
+  /* MCVD_OP_CONV3D on the TF32 tensor cores (wgmma m64nNk8 tf32, fp32 accumulators; mcvd_b200/csrc/conv_tf32.cu).
+   * Every field and the geometry contract are MCVD_OP_CONV3D's, except w: the packed TF32 image of the
+   * [i0][i1][i1][C0][Cout] weights that mcvd_tf32_pack_weights(w, K = i0 * i1 * i1 * C0, Cout, ...) writes.
+   * Activations are rounded once to TF32 with round-to-nearest, ties away from zero (cvt.rna) as they are staged,
+   * the weights the same way when packed; the products are exact and summed in fp32.  The result differs from
+   * MCVD_OP_CONV3D's by the TF32 rounding of both operands (a relative 2^-11 each).  Each output is accumulated in
+   * one fixed K order: a video's features do not depend on the batch or chunk it is computed in. */
+  MCVD_OP_CONV3D_TF32 = 34,
+  /* MCVD_OP_CONV2D on the TF32 tensor cores: every field, flag (MCVD_F_POOL, MCVD_F_AVG) and the geometry contract
+   * are MCVD_OP_CONV2D's, except w: the packed TF32 image of the [i0][i1][C0][Cout] weights,
+   * mcvd_tf32_pack_weights(w, K = i0 * i1 * C0, Cout, ...).  The fused pool is formed in fp32 and rounded once.
+   * Numerics as MCVD_OP_CONV3D_TF32. */
+  MCVD_OP_CONV2D_TF32 = 35,
   MCVD_OP__COUNT
 };
 
@@ -344,6 +357,13 @@ long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cout);
  * this call fills (taps*Cin*Cout*4); out == NULL only queries. */
 long long mcvd_umma2_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int k_block,
                                   void* out, int scale_log2, int stage_off, int per_unit, void* stream);
+/* Packed TF32 weights of MCVD_OP_CONV3D_TF32 / MCVD_OP_CONV2D_TF32.  w_kmajor = fp32 [K][Cout] on the device (the
+ * MCVD_OP_CONV3D / MCVD_OP_CONV2D layout; K = taps * Cin, Cout a positive multiple of 8); out = device buffer of
+ * mcvd_tf32_packed_bytes(K, Cout) bytes, 16-byte aligned, written on `stream`.  Every value is rounded to TF32
+ * (round to nearest, ties away from zero); the layout (n tiles and K slabs padded with zeros) belongs to the library.
+ * mcvd_tf32_packed_bytes returns < 0 for an unusable K / Cout; mcvd_tf32_pack_weights returns 0 or < 0. */
+long long mcvd_tf32_packed_bytes(int K, int Cout);
+int mcvd_tf32_pack_weights(const float* w_kmajor, int K, int Cout, void* out, void* stream);
 /* Bytes of dst2 scratch one MCVD_OP_ATTENTION_UMMA op with batch B, T = H*W tokens and C channels needs. */
 long long mcvd_attention_scratch_bytes(int B, int T, int C);
 

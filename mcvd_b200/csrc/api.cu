@@ -50,6 +50,8 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_FID_HEAD: return launch_fid_head(op, s);
     case MCVD_OP_KNN_RADIUS:
     case MCVD_OP_KNN_COVER: return launch_knn(op, s);
+    case MCVD_OP_CONV3D_TF32: return launch_conv3d_tf32(op, s);
+    case MCVD_OP_CONV2D_TF32: return launch_conv2d_tf32(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -201,6 +203,19 @@ static int validate_one(const McvdOp& op, int idx) {
       }
       if (misaligned(op.bias)) {
         set_error("op %d %s: bias must be 16-byte aligned", idx, names[op.kind - MCVD_OP_FID_PREP]);
+        return -1;
+      }
+      break;
+    }
+    case MCVD_OP_CONV3D_TF32:
+    case MCVD_OP_CONV2D_TF32: {
+      const char* name = op.kind == MCVD_OP_CONV3D_TF32 ? "CONV3D_TF32" : "CONV2D_TF32";
+      if (const char* why = conv_tf32_error(op)) {
+        set_error("op %d %s: %s", idx, name, why);
+        return -1;
+      }
+      if (misaligned(op.bias)) {
+        set_error("op %d %s: bias must be 16-byte aligned", idx, name);
         return -1;
       }
       break;

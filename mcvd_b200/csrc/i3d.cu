@@ -10,16 +10,6 @@ namespace mcvd {
 
 constexpr int I3D_SIDE = 224;
 
-// TF-"SAME" padding of one axis (pytorch_i3d.py compute_pad): the total; the front gets total / 2
-__host__ __device__ inline int same_pad(int in, int k, int s) {
-  const int r = in % s;
-  const int p = r == 0 ? k - s : k - r;
-  return p > 0 ? p : 0;
-}
-
-// output extent of one axis after SAME padding: (in + pad - k) / s + 1, which is ceil(in / s) for I3D's shapes
-__host__ __device__ inline int same_out(int in, int k, int s) { return (in + same_pad(in, k, s) - k) / s + 1; }
-
 // ------------------------------------------------------------------------------------------------
 // prep: bilinear resize (ATen's align_corners=False source index), centre crop to 224x224, (x - 0.5) * 2; a grey
 // frame is replicated to RGB and channel 3 is zero.  One thread per output pixel of one frame.

@@ -30,6 +30,16 @@ void set_error(const char* fmt, ...);
 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
+// TF-"SAME" padding of one axis (pytorch_i3d.py compute_pad): the total; the front gets total / 2
+__host__ __device__ inline int same_pad(int in, int k, int s) {
+  const int r = in % s;
+  const int p = r == 0 ? k - s : k - r;
+  return p > 0 ? p : 0;
+}
+
+// output extent of one axis after SAME padding: (in + pad - k) / s + 1, which is ceil(in / s) for I3D's shapes
+__host__ __device__ inline int same_out(int in, int k, int s) { return (in + same_pad(in, k, s) - k) / s + 1; }
+
 __device__ __forceinline__ float silu_f(float v) { return v / (1.0f + expf(-v)); }
 
 // launchers (one per op kind); each returns 0 or a negative error code
@@ -84,6 +94,12 @@ const char* conv2d_error(const McvdOp& op);
 const char* maxpool2d_error(const McvdOp& op);
 const char* fid_head_error(const McvdOp& op);
 const char* knn_error(const McvdOp& op);
+
+// MCVD_OP_CONV3D_TF32 / MCVD_OP_CONV2D_TF32 (conv_tf32.cu): NULL, or why the op is unusable (shared by validation and
+// launch), and the launchers
+const char* conv_tf32_error(const McvdOp& op);
+int launch_conv3d_tf32(const McvdOp& op, cudaStream_t s);
+int launch_conv2d_tf32(const McvdOp& op, cudaStream_t s);
 
 // NULL, or why the Gamma parameters (f6 = shape, f7 = scale) of an op with MCVD_F_GAMMA are unusable
 const char* gamma_params_error(const McvdOp& op);

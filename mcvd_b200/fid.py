@@ -10,6 +10,9 @@ set that falls inside the k-NN balls (k = 3) of the other.
 ``InceptionV3`` computes the features for whole chunks of frames with the library's own kernels
 (``MCVD_OP_FID_PREP``, ``MCVD_OP_CONV2D``, ``MCVD_OP_MAXPOOL2D``, ``MCVD_OP_FID_HEAD``): ``LAUNCHES_PER_CHUNK``
 launches per chunk, whatever its size; a frame's features do not depend on the batch or chunk it is computed in.
+``InceptionV3(..., tf32=True)`` runs the convolutions on the TF32 tensor cores instead (``MCVD_OP_CONV2D_TF32``):
+both operands rounded once to TF32, fp32 accumulation, the numerics class of cuDNN with ``allow_tf32``.  The drop-ins
+use it when the environment sets ``MCVD_EVAL_TF32=1``; by default they keep the fp32 path.
 Grey frames are accepted (replicated to RGB); the reference raises on them.  ``precision_recall`` runs
 ``MCVD_OP_KNN_RADIUS`` and ``MCVD_OP_KNN_COVER`` (four launches) and never forms the N x N distance matrix the
 reference moves to the host; its distances are exact differences, so a point's distance to itself is 0.
@@ -279,15 +282,27 @@ class InceptionV3:
     Batch norm is folded and the weights are packed once, onto ``device`` (default: the current CUDA device).
     Frames are processed in chunks of at most ``max_chunk_frames``; a chunk needs ``workspace_floats() * 4`` bytes
     (10.2 MB) per frame, so the default (``DEFAULT_CHUNK`` = 210 frames) keeps it under 2 GiB.
+
+    ``tf32``: run the 94 convolutions on the TF32 tensor cores (``MCVD_OP_CONV2D_TF32``).  Activations (after the
+    fused branch pools) and weights are rounded once to TF32 (round to nearest, ties away from zero) and the products
+    summed in fp32, so the features differ from the default fp32 ones by about the TF32 rounding (cuDNN's
+    ``allow_tf32`` class of numerics); a frame's features still do not depend on its batch or chunk.  The packed TF32
+    weights are made once here and take 90.8 MB of device memory on top of the 87.0 MB of folded fp32 weights.  The
+    default (False) is the fp32 FFMA path, unchanged.
     """
 
     def __init__(self, state_dict_or_path, device: Optional[Union[str, torch.device]] = None,
-                 max_chunk_frames: int = DEFAULT_CHUNK):
+                 max_chunk_frames: int = DEFAULT_CHUNK, tf32: bool = False):
         if not 1 <= int(max_chunk_frames) <= 65535:
             raise ValueError(f"InceptionV3: max_chunk_frames={max_chunk_frames} must be in [1, 65535]")
         self.device = torch.device(device if device is not None else "cuda")
         self.max_chunk_frames = int(max_chunk_frames)
         self.weights = {k: tuple(t.to(self.device) for t in v) for k, v in pack_weights(state_dict_or_path).items()}
+        self.tf32 = bool(tf32)
+        self.packed = {}
+        if self.tf32:
+            from . import lib
+            self.packed = {key: lib.tf32_pack_weights(self.weights[key][0]) for key, _, _, _ in units()}
 
     def program(self, frames: torch.Tensor, out: torch.Tensor, ws: torch.Tensor):
         """The ops of one chunk: ``frames`` [n, C, S, S] fp32 CUDA, ``out`` fp64 [n, 2048], ``ws`` at least
@@ -315,8 +330,11 @@ class InceptionV3:
                 op.src0, op.dst = bufs[st["src"]].data_ptr(), bufs[st["dst"]].data_ptr()
             else:
                 w, b = self.weights[st["key"]]
+                if self.tf32:
+                    w = self.packed[st["key"]]
                 (kh, kw), (ph, pw) = st["k"], st["pad"]
-                op.kind, op.C0, op.Cout = lib.OP_CONV2D, st["c"], st["cout"]
+                op.kind = lib.OP_CONV2D_TF32 if self.tf32 else lib.OP_CONV2D
+                op.C0, op.Cout = st["c"], st["cout"]
                 op.H, op.W = conv_out(st["s"], kh, st["stride"], ph), conv_out(st["s"], kw, st["stride"], pw)
                 op.i0, op.i1, op.i2, op.i3, op.i4, op.i5 = kh, kw, st["stride"], ph, pw, st["s"]
                 op.i6, op.i7 = st["pitch"], st["off"]
@@ -484,12 +502,18 @@ def native_unsupported(device, dims) -> Optional[str]:
 
 
 @functools.lru_cache(maxsize=2)
-def _model(path: str, device: str) -> InceptionV3:
-    return InceptionV3(path, device=device)
+def _model(path: str, device: str, tf32: bool = False) -> InceptionV3:
+    return InceptionV3(path, device=device, tf32=tf32)
+
+
+def env_tf32() -> bool:
+    """True when ``MCVD_EVAL_TF32=1``: the drop-ins then compute features on the TF32 tensor cores."""
+    return os.environ.get("MCVD_EVAL_TF32", "0") == "1"
 
 
 def model_for(device) -> InceptionV3:
-    """The ``InceptionV3`` of the hub-cache weights on ``device``, built once per process."""
+    """The ``InceptionV3`` of the hub-cache weights on ``device``, built once per process (and per ``MCVD_EVAL_TF32``
+    setting: with ``MCVD_EVAL_TF32=1`` it runs its convolutions in TF32)."""
     path = default_weights_path()
     if not os.path.exists(path):
         raise FileNotFoundError(f"FID weights not found at {path}; mcvd_b200 never downloads them (place "
@@ -497,7 +521,7 @@ def model_for(device) -> InceptionV3:
     dev = torch.device(device)
     if dev.type == "cuda" and dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    return _model(path, str(dev))
+    return _model(path, str(dev), env_tf32())
 
 
 def _check_dims(dims):

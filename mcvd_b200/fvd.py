@@ -9,6 +9,8 @@ video's feature and compares the feature sets of fake and real videos with the F
 ``I3D`` computes the same features for whole batches with the library's own kernels (``MCVD_OP_I3D_PREP``,
 ``MCVD_OP_CONV3D``, ``MCVD_OP_MAXPOOL3D``, ``MCVD_OP_I3D_HEAD``): ``LAUNCHES_PER_CHUNK`` launches per chunk of
 videos, whatever its size.  A video's features do not depend on the batch or chunk it is computed in.
+``I3D(..., tf32=True)`` runs the convolutions on the TF32 tensor cores instead (``MCVD_OP_CONV3D_TF32``): both
+operands rounded once to TF32, fp32 accumulation, the numerics class of cuDNN with ``allow_tf32``.
 
 Weights are never downloaded.  ``I3D`` takes an ``InceptionI3d`` state_dict (``Conv3d_1a_7x7.conv3d.weight``,
 ``Conv3d_1a_7x7.bn.{weight,bias,running_mean,running_var}``, ``Mixed_3b.b1b.conv3d.weight``, ...,
@@ -201,15 +203,27 @@ class I3D:
     weights are packed once, onto ``device`` (default: the current CUDA device).  Videos are processed in chunks of
     at most ``max_chunk_videos``; a chunk needs ``workspace_floats(T) * 4`` bytes per video (33 MiB at T = 10,
     86 MiB at T = 25, 99 MiB at T = 30), so the default of 16 keeps it under 1.6 GiB up to T = 30.
+
+    ``tf32``: run the 57 convolutions on the TF32 tensor cores (``MCVD_OP_CONV3D_TF32``).  Activations and weights
+    are rounded once to TF32 (round to nearest, ties away from zero) and the products summed in fp32, so the features
+    differ from the default fp32 ones by about the TF32 rounding (cuDNN's ``allow_tf32`` class of numerics); a video's
+    features still do not depend on its batch or chunk.  The packed TF32 weights are made once here and take 52.9 MB
+    of device memory on top of the 49.2 MB of folded fp32 weights.  The default (False) is the fp32 FFMA path,
+    unchanged.
     """
 
     def __init__(self, state_dict_or_path, device: Optional[Union[str, torch.device]] = None,
-                 max_chunk_videos: int = 16):
+                 max_chunk_videos: int = 16, tf32: bool = False):
         if not 1 <= int(max_chunk_videos) <= 4096:
             raise ValueError(f"I3D: max_chunk_videos={max_chunk_videos} must be in [1, 4096]")
         self.device = torch.device(device if device is not None else "cuda")
         self.max_chunk_videos = int(max_chunk_videos)
         self.weights = {k: tuple(t.to(self.device) for t in v) for k, v in pack_weights(state_dict_or_path).items()}
+        self.tf32 = bool(tf32)
+        self.packed = {}
+        if self.tf32:
+            from . import lib
+            self.packed = {key: lib.tf32_pack_weights(self.weights[key][0]) for key, _, _, _ in units()}
 
     def program(self, videos: torch.Tensor, channels: int, out: torch.Tensor, ws: torch.Tensor):
         """The ops of one chunk: ``videos`` [n, channels*T, S, S] fp32 CUDA, ``out`` fp64 [n, 400], ``ws`` at least
@@ -246,7 +260,10 @@ class I3D:
                     op.kind = lib.OP_MAXPOOL3D
                 else:
                     w, b = self.weights[st["key"]]
-                    op.kind, op.Cout, op.i6, op.i7 = lib.OP_CONV3D, st["cout"], st["pitch"], st["off"]
+                    if self.tf32:
+                        w = self.packed[st["key"]]
+                    op.kind = lib.OP_CONV3D_TF32 if self.tf32 else lib.OP_CONV3D
+                    op.Cout, op.i6, op.i7 = st["cout"], st["pitch"], st["off"]
                     op.w, op.bias = w.data_ptr(), b.data_ptr()
             ops.append(op)
         return ops

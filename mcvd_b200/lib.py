@@ -45,6 +45,8 @@ OP_MAXPOOL2D = 30
 OP_FID_HEAD = 31
 OP_KNN_RADIUS = 32
 OP_KNN_COVER = 33
+OP_CONV3D_TF32 = 34
+OP_CONV2D_TF32 = 35
 
 F_ACT_IN = 1 << 0
 F_ACT_OUT = 1 << 1
@@ -63,7 +65,8 @@ ABI_VERSION = 5
 
 EXPORTS = ["mcvd_abi_version", "mcvd_sizeof_op", "mcvd_last_error", "mcvd_device_arch", "mcvd_run_program",
            "mcvd_validate_program", "mcvd_count_launches", "mcvd_umma_pack_weights", "mcvd_umma_kblock",
-           "mcvd_attention_scratch_bytes", "mcvd_umma2_plan", "mcvd_umma2_plan_info", "mcvd_umma2_stats_bytes", "mcvd_umma2_pack_weights"]
+           "mcvd_attention_scratch_bytes", "mcvd_umma2_plan", "mcvd_umma2_plan_info", "mcvd_umma2_stats_bytes", "mcvd_umma2_pack_weights",
+           "mcvd_tf32_packed_bytes", "mcvd_tf32_pack_weights"]
 
 
 class McvdOp(C.Structure):
@@ -141,6 +144,10 @@ def load():
         lib.mcvd_umma2_pack_weights.restype = C.c_longlong
         lib.mcvd_umma2_pack_weights.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                                 C.c_int, C.c_int, C.c_int, C.c_void_p]
+        lib.mcvd_tf32_packed_bytes.restype = C.c_longlong
+        lib.mcvd_tf32_packed_bytes.argtypes = [C.c_int, C.c_int]
+        lib.mcvd_tf32_pack_weights.restype = C.c_int
+        lib.mcvd_tf32_pack_weights.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         if lib.mcvd_abi_version() != ABI_VERSION:
             raise RuntimeError("mcvd_b200: ABI version mismatch between the Python binding and the library")
         if lib.mcvd_sizeof_op() != C.sizeof(McvdOp):
@@ -207,3 +214,29 @@ def umma2_pick_nt(cout: int, ks: int) -> int:
         if cout % d == 0:
             best = d
     return best
+
+
+def tf32_packed_bytes(K: int, cout: int) -> int:
+    """bytes of the packed TF32 weight image of a [K, Cout] convolution (OP_CONV3D_TF32 / OP_CONV2D_TF32); host
+    arithmetic only"""
+    n = int(load().mcvd_tf32_packed_bytes(K, cout))
+    if n < 0:
+        raise RuntimeError(f"mcvd_b200 tf32_packed_bytes failed: {last_error()}")
+    return n
+
+
+def tf32_pack_weights(w):
+    """The packed TF32 image (``w`` of OP_CONV3D_TF32 / OP_CONV2D_TF32) of folded weights ``w`` fp32 [K, Cout] on a
+    CUDA device, as an fp32 tensor on the same device.  The layout belongs to the library."""
+    import torch
+    if w.device.type != "cuda" or w.dtype != torch.float32 or w.dim() != 2:
+        raise ValueError(f"tf32_pack_weights: weights must be fp32 [K, Cout] on CUDA, got {w.dtype} "
+                         f"{tuple(w.shape)} on {w.device}")
+    w = w.contiguous()
+    K, cout = w.shape
+    out = torch.empty(tf32_packed_bytes(K, cout) // 4, dtype=torch.float32, device=w.device)
+    with torch.cuda.device(w.device):
+        stream = torch.cuda.current_stream(w.device).cuda_stream
+        check(load().mcvd_tf32_pack_weights(w.data_ptr(), K, cout, out.data_ptr(), C.c_void_p(stream)),
+              "tf32_pack_weights")
+    return out

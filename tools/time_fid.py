@@ -1,11 +1,12 @@
 """Time FID's Inception features and k-NN precision / recall (mcvd_b200.fid) on the GPU against torch baselines.
 
-    python tools/time_fid.py [--reps 5] [--frames 2000] [--cases cfg2,cfg4,cfg5] [--pr 10000,50000]
+    python tools/time_fid.py [--reps 5] [--frames 2000] [--cases cfg2,cfg4,cfg5] [--pr 10000,50000] [--profile DIR]
 
 Features: frame sets shaped like the benchmark workloads' ``fast_fid`` output, with synthetic weights
 (``oracle.inception_oracle.synthetic_weights``) and random frames:
   * cfg2: 64x64, 1 channel;  cfg4: 64x64, 3 channels;  cfg5: 128x128, 3 channels.
-``native`` is the whole ``InceptionV3`` call (prep, 94 convolutions, 4 pools, head) with the default chunk.
+``native`` is the whole ``InceptionV3`` call (prep, 94 convolutions, 4 pools, head) with the default chunk, fp32 FFMA
+convolutions; ``native_tf32`` the same with ``tf32=True`` (TF32 wgmma convolutions).
 ``cudnn`` is ``F.interpolate`` + ``F.conv2d`` / pools with the same folded weights, in chunks of the same size, with
 TF32 off and on.  FLOPs are counted from the shapes (2 per multiply-add of the convolutions).
 
@@ -17,6 +18,8 @@ half of the host's free memory.
 
 Each measurement is timed with CUDA events around work that ends in a synchronise, after a warm-up, alternated
 ``--reps`` times; the median is reported.  Prints the GPU's name and power limit, then one JSON line per case.
+``--profile DIR``: afterwards, one ``native_tf32`` call per case under ``torch.profiler`` (a run of its own), with the
+summed CUDA time per kernel name printed and the trace written to DIR.
 """
 import argparse
 import json
@@ -117,18 +120,42 @@ def median_times(runs, reps):
     return {k: statistics.median(v) for k, v in times.items()}
 
 
+def profile_kernels(fn, out_dir, tag):
+    """One call of ``fn`` under torch.profiler: prints the summed CUDA time per kernel and writes the trace."""
+    from torch.profiler import ProfilerActivity, profile
+    os.makedirs(out_dir, exist_ok=True)
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    prof.export_chrome_trace(os.path.join(out_dir, f"{tag}.pt.trace.json"))
+    per = {}
+    for e in prof.events():
+        if e.device_type == torch.autograd.DeviceType.CUDA:
+            k = e.name.split("(")[0][:90]
+            n, t = per.get(k, (0, 0.0))
+            per[k] = (n + 1, t + e.device_time_total / 1e3)
+    total = sum(t for _, t in per.values())
+    rows = sorted(per.items(), key=lambda kv: -kv[1][1])[:12]
+    print(json.dumps({"profile": tag, "kernel_ms_total": round(total, 2),
+                      "top": [[k, n, round(t, 2)] for k, (n, t) in rows]}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--frames", type=int, default=2000)
     ap.add_argument("--cases", default=",".join(CASES))
     ap.add_argument("--pr", default="10000,50000")
+    ap.add_argument("--profile", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "time_fid.py measures on a CUDA device"
     dev = torch.device("cuda", torch.cuda.current_device())
     print(f"# {torch.cuda.get_device_name(dev)}, power limit {power_limit_w()} W", flush=True)
     sd = NO.synthetic_weights()
     net = FD.InceptionV3(sd, device=dev)
+    net_tf32 = FD.InceptionV3(sd, device=dev, tf32=True)
     ref = TorchInception(sd, dev)
     chunk = net.max_chunk_frames
     g = torch.Generator(device=dev).manual_seed(0)
@@ -141,7 +168,7 @@ def main():
             with torch.no_grad():
                 return torch.cat([ref(frames[lo:lo + chunk]) for lo in range(0, N, chunk)])
 
-        runs = {"native": lambda: net(frames, C)}
+        runs = {"native": lambda: net(frames, C), "native_tf32": lambda: net_tf32(frames, C)}
         for tf32 in (False, True):
             runs[f"cudnn_tf32_{'on' if tf32 else 'off'}"] = (lambda t=tf32: (
                 setattr(torch.backends.cudnn, "allow_tf32", t), setattr(torch.backends.cuda.matmul, "allow_tf32", t),
@@ -152,15 +179,23 @@ def main():
         for k, ms in med.items():
             res[f"{k}_ms"] = round(ms, 1)
             res[f"{k}_tflops"] = round(flops / ms / 1e9, 2)
-        f_native = net(frames, C)
+        f_native, f_tf32 = net(frames, C), net_tf32(frames, C)
+        torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = True
+        f_ref_tf32 = torch_run()
         torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
         f_ref = torch_run()
         res["max_abs_diff_vs_cudnn_fp32_over_scale"] = float((f_native - f_ref).abs().max() / f_ref.abs().max())
+        res["native_tf32_vs_native_over_scale"] = float((f_tf32 - f_native).abs().max() / f_native.abs().max())
+        res["cudnn_tf32_vs_cudnn_fp32_over_scale"] = float((f_ref_tf32 - f_ref).abs().max() / f_ref.abs().max())
         half = N // 2
         res["fid_native"] = FD.fid(f_native[half:], f_native[:half])
+        res["fid_native_tf32"] = FD.fid(f_tf32[half:], f_tf32[:half])
         res["fid_cudnn_fp32"] = FD.fid(f_ref[half:], f_ref[:half])
+        res["fid_cudnn_tf32"] = FD.fid(f_ref_tf32[half:], f_ref_tf32[:half])
         print(json.dumps(res), flush=True)
-        del frames, f_native, f_ref
+        if args.profile:
+            profile_kernels(lambda: net_tf32(frames, C), args.profile, name)
+        del frames, f_native, f_tf32, f_ref, f_ref_tf32
         torch.cuda.empty_cache()
     for n in [int(v) for v in args.pr.split(",") if v]:
         real = torch.relu(torch.randn(n, 2048, device=dev, generator=g))

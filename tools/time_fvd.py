@@ -1,17 +1,20 @@
 """Time FVD's I3D features (mcvd_b200.fvd.I3D) on the GPU against the same network in cuDNN.
 
-    python tools/time_fvd.py [--reps 5] [--cases cfg2,cfg4,cfg5]
+    python tools/time_fvd.py [--reps 5] [--cases cfg2,cfg4,cfg5] [--profile DIR]
 
 The video sets of the benchmark workloads' FVD (real plus fake videos, one prediction per test clip), with synthetic
 weights (``oracle.i3d_oracle.synthetic_weights``) and synthetic videos:
   * cfg2: 64 + 64 videos of 25 frames (5 conditioning + 20 predicted), 64x64, 1 channel;
   * cfg4: 64 + 64 videos of 30 frames (2 + 28), 64x64, 3 channels;
   * cfg5: 32 + 32 videos of 30 frames (2 + 28), 128x128, 3 channels.
-``native`` is the whole ``I3D`` call (prep, 57 convolutions, 13 pools, head) with the default chunk of 16 videos.
+``native`` is the whole ``I3D`` call (prep, 57 convolutions, 13 pools, head) with the default chunk of 16 videos, fp32
+FFMA convolutions; ``native_tf32`` the same with ``tf32=True`` (TF32 wgmma convolutions).
 ``cudnn`` is ``F.interpolate`` + ``F.conv3d`` / ``F.max_pool3d`` / ``F.avg_pool3d`` with the same folded weights, in
 chunks of 16 videos, with TF32 off and on.  Each is timed with CUDA events after a warm-up, alternated ``--reps``
 times; the median is reported.  FLOPs are counted from the shapes (2 per multiply-add of the convolutions and the
-logits).  Prints the GPU's name and power limit, then one JSON line per case.
+logits).  Prints the GPU's name and power limit, then one JSON line per case.  ``--profile DIR``: afterwards, one
+``native_tf32`` call per case under ``torch.profiler`` (a run of its own), with the summed CUDA time per kernel name
+printed and the trace written to DIR.
 """
 import argparse
 import json
@@ -26,6 +29,7 @@ import torch.nn.functional as Fn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from mcvd_b200 import fvd as FV  # noqa: E402
 from oracle import i3d_oracle as IO  # noqa: E402
+from tools.time_fid import profile_kernels  # noqa: E402
 
 CASES = {"cfg2": (64, 25, 64, 1), "cfg4": (64, 30, 64, 3), "cfg5": (32, 30, 128, 3)}
 
@@ -111,12 +115,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--cases", default=",".join(CASES))
+    ap.add_argument("--profile", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "time_fvd.py measures on a CUDA device"
     dev = torch.device("cuda", torch.cuda.current_device())
     print(f"# {torch.cuda.get_device_name(dev)}, power limit {power_limit_w()} W", flush=True)
     sd = IO.synthetic_weights()
     net = FV.I3D(sd, device=dev)
+    net_tf32 = FV.I3D(sd, device=dev, tf32=True)
     ref = CudnnI3D(sd, dev)
     g = torch.Generator(device=dev).manual_seed(0)
     for name in args.cases.split(","):
@@ -130,7 +136,7 @@ def main():
             with torch.no_grad():
                 return torch.cat([ref(videos[lo:lo + 16], C) for lo in range(0, N, 16)])
 
-        runs = {"native": lambda: net(videos, C)}
+        runs = {"native": lambda: net(videos, C), "native_tf32": lambda: net_tf32(videos, C)}
         for tf32 in (False, True):
             runs[f"cudnn_tf32_{'on' if tf32 else 'off'}"] = (lambda t=tf32: (
                 setattr(torch.backends.cudnn, "allow_tf32", t), setattr(torch.backends.cuda.matmul, "allow_tf32", t),
@@ -147,13 +153,21 @@ def main():
             ms = statistics.median(ts)
             res[f"{k}_ms"] = round(ms, 2)
             res[f"{k}_tflops"] = round(flops / ms / 1e9, 2)
-        f_native = net(videos, C)
+        f_native, f_tf32 = net(videos, C), net_tf32(videos, C)
+        torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = True
+        f_ref_tf32 = cudnn_run()
         torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
         f_ref = cudnn_run()
         res["max_abs_diff_vs_cudnn_fp32_over_scale"] = float((f_native - f_ref).abs().max() / f_ref.abs().max())
+        res["native_tf32_vs_native_over_scale"] = float((f_tf32 - f_native).abs().max() / f_native.abs().max())
+        res["cudnn_tf32_vs_cudnn_fp32_over_scale"] = float((f_ref_tf32 - f_ref).abs().max() / f_ref.abs().max())
         res["fvd_native"] = FV.frechet_distance(f_native[B:], f_native[:B])
+        res["fvd_native_tf32"] = FV.frechet_distance(f_tf32[B:], f_tf32[:B])
         res["fvd_cudnn_fp32"] = FV.frechet_distance(f_ref[B:], f_ref[:B])
+        res["fvd_cudnn_tf32"] = FV.frechet_distance(f_ref_tf32[B:], f_ref_tf32[:B])
         print(json.dumps(res), flush=True)
+        if args.profile:
+            profile_kernels(lambda: net_tf32(videos, C), args.profile, name)
 
 
 if __name__ == "__main__":
