@@ -54,6 +54,17 @@ def _ptr(t) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def umma_scale_log2(amax: float) -> int:
+    """Power-of-two pre-scale k of a tensor-core conv's weights (the kernel multiplies by f1 = 2^-k afterwards):
+    max|w| * 2^k lies in [256, 512), so the fp16 hi parts keep 11 bits and the lo parts stay in the fp16 normal range
+    down to 2^-25 of the layer's largest weight, and nothing saturates, whatever the layer's scale.  |k| <= 126 keeps
+    2^k and 2^-k normal fp32 numbers (only max|w| < 2^-117 then lands below 256).  An earlier floor(log2(512 / max|w|))
+    clamped to |k| <= 24 chose the same k except when max|w| is an exact power of two, which it scaled to 512."""
+    if amax == 0.0 or not math.isfinite(amax):
+        return 0
+    return max(-126, min(126, 9 - math.frexp(amax)[1]))
+
+
 def _pick_nt(cout: int) -> int:
     best = 0
     for d in range(16, 257, 16):
@@ -244,9 +255,7 @@ class Engine:
             return self.backend.pack_umma(taps, nt, kb)
         self.packs_computed += 1
         T, I, O = taps.shape
-        amax = float(taps.abs().max().item())
-        k = 0 if amax == 0.0 else int(math.floor(math.log2(512.0 / amax)))
-        k = max(-24, min(24, k))
+        k = umma_scale_log2(float(taps.abs().max().item()))
         out = torch.empty(T * I * O * 4, device=taps.device, dtype=torch.uint8)
         stream = self._stream()
         with self._devctx():
@@ -262,9 +271,7 @@ class Engine:
             t, _ = self.backend.pack_umma(both, nt, kb)
             return t, 1.0
         self.packs_computed += 1
-        amax = float(max(taps.abs().max().item(), taps_sc.abs().max().item()))
-        k = 0 if amax == 0.0 else int(math.floor(math.log2(512.0 / amax)))
-        k = max(-24, min(24, k))
+        k = umma_scale_log2(float(max(taps.abs().max().item(), taps_sc.abs().max().item())))
         n_nt = taps.shape[2] // nt
         parts = []
         for t in (taps, taps_sc):
@@ -287,8 +294,7 @@ class Engine:
         amax = float(taps.abs().max().item())
         if taps_sc is not None:
             amax = max(amax, float(taps_sc.abs().max().item()))
-        k = 0 if amax == 0.0 else int(math.floor(math.log2(512.0 / amax)))
-        k = max(-24, min(24, k))
+        k = umma_scale_log2(amax)
         T, I, O = taps.shape
         isc = 0 if taps_sc is None else taps_sc.shape[1]
         per_unit = (I // kb) * T + isc // kb
