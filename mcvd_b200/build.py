@@ -16,8 +16,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(LIBDIR, "libmcvd_b200.so")
 SOURCES = ["api.cu", "elementwise.cu", "conv_simt.cu", "conv_smalln.cu", "attention_simt.cu", "conv_umma.cu",
-           "attention_umma.cu", "lpips.cu", "i3d.cu", "dsm.cu", "inception.cu", "knn.cu", "conv_tf32.cu"]
-HEADERS = [os.path.join(CSRC, "mcvd_common.cuh"), os.path.join(CSRC, "philox.cuh"), os.path.join(CSRC, "umma_ptx.cuh"), os.path.join(CSRC, "wgmma_ops.cuh"), os.path.join(os.path.dirname(HERE), "include", "mcvd_b200.h")]
+           "attention_umma.cu", "lpips.cu", "i3d.cu", "dsm.cu", "inception.cu", "knn.cu", "conv_eval.cu", "conv_tf32.cu"]
+HEADERS = [os.path.join(CSRC, "mcvd_common.cuh"), os.path.join(CSRC, "conv_eval.cuh"), os.path.join(CSRC, "philox.cuh"), os.path.join(CSRC, "umma_ptx.cuh"), os.path.join(CSRC, "wgmma_ops.cuh"), os.path.join(os.path.dirname(HERE), "include", "mcvd_b200.h")]
 
 
 def _nvcc() -> str:

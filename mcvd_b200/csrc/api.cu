@@ -2,7 +2,7 @@
 #include <stdarg.h>
 #include <string.h>
 
-#include "mcvd_common.cuh"
+#include "conv_eval.cuh"
 
 namespace mcvd {
 
@@ -36,22 +36,22 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_FRAME_METRICS: return launch_frame_metrics(op, s);
     case MCVD_OP_NOISE: return launch_noise(op, s);
     case MCVD_OP_LPIPS_PREP: return launch_lpips_prep(op, s);
-    case MCVD_OP_CONV_RELU: return launch_conv_relu(op, s);
+    case MCVD_OP_CONV_RELU:
+    case MCVD_OP_CONV3D:
+    case MCVD_OP_CONV2D: return launch_conv_ffma(op, s);
+    case MCVD_OP_MAXPOOL3D:
+    case MCVD_OP_MAXPOOL2D: return launch_maxpool(op, s);
+    case MCVD_OP_CONV3D_TF32:
+    case MCVD_OP_CONV2D_TF32: return launch_conv_tf32(op, s);
     case MCVD_OP_LPIPS_LAYER: return launch_lpips_layer(op, s);
     case MCVD_OP_I3D_PREP: return launch_i3d_prep(op, s);
-    case MCVD_OP_CONV3D: return launch_conv3d(op, s);
-    case MCVD_OP_MAXPOOL3D: return launch_maxpool3d(op, s);
     case MCVD_OP_I3D_HEAD: return launch_i3d_head(op, s);
     case MCVD_OP_DSM_PERTURB: return launch_dsm_perturb(op, s);
     case MCVD_OP_DSM_LOSS: return launch_dsm_loss(op, s);
     case MCVD_OP_FID_PREP: return launch_fid_prep(op, s);
-    case MCVD_OP_CONV2D: return launch_conv2d(op, s);
-    case MCVD_OP_MAXPOOL2D: return launch_maxpool2d(op, s);
     case MCVD_OP_FID_HEAD: return launch_fid_head(op, s);
     case MCVD_OP_KNN_RADIUS:
     case MCVD_OP_KNN_COVER: return launch_knn(op, s);
-    case MCVD_OP_CONV3D_TF32: return launch_conv3d_tf32(op, s);
-    case MCVD_OP_CONV2D_TF32: return launch_conv2d_tf32(op, s);
     default: break;
   }
   set_error("unknown op kind %d", op.kind);
@@ -144,15 +144,24 @@ static int validate_one(const McvdOp& op, int idx) {
       }
       break;
     case MCVD_OP_CONV_RELU:
-      if (const char* why = conv_relu_error(op)) {
-        set_error("op %d CONV_RELU: %s", idx, why);
+    case MCVD_OP_CONV3D:
+    case MCVD_OP_MAXPOOL3D:
+    case MCVD_OP_CONV2D:
+    case MCVD_OP_MAXPOOL2D:
+    case MCVD_OP_CONV3D_TF32:
+    case MCVD_OP_CONV2D_TF32: {
+      ConvGeom g;
+      const bool tf32 = op.kind == MCVD_OP_CONV3D_TF32 || op.kind == MCVD_OP_CONV2D_TF32;
+      if (const char* why = tf32 ? conv_tf32_geom(op, g) : conv_geom(op, g)) {
+        set_error("op %d %s: %s", idx, conv_kind_name(op.kind), why);
         return -1;
       }
       if (misaligned(op.bias)) {
-        set_error("op %d CONV_RELU: bias must be 16-byte aligned", idx);
+        set_error("op %d %s: bias must be 16-byte aligned", idx, conv_kind_name(op.kind));
         return -1;
       }
       break;
+    }
     case MCVD_OP_LPIPS_LAYER:
       if (!op.src1 || !op.w || op.C0 < 1) {
         set_error("op %d LPIPS_LAYER: null real features or lin weights, or %d channels", idx, op.C0);
@@ -160,20 +169,14 @@ static int validate_one(const McvdOp& op, int idx) {
       }
       break;
     case MCVD_OP_I3D_PREP:
-    case MCVD_OP_CONV3D:
-    case MCVD_OP_MAXPOOL3D:
     case MCVD_OP_I3D_HEAD: {
-      const char* why = op.kind == MCVD_OP_I3D_PREP ? i3d_prep_error(op)
-                        : op.kind == MCVD_OP_CONV3D  ? conv3d_error(op)
-                        : op.kind == MCVD_OP_MAXPOOL3D ? maxpool3d_error(op)
-                                                       : i3d_head_error(op);
-      static const char* const names[] = {"I3D_PREP", "CONV3D", "MAXPOOL3D", "I3D_HEAD"};
-      if (why) {
-        set_error("op %d %s: %s", idx, names[op.kind - MCVD_OP_I3D_PREP], why);
+      const char* name = op.kind == MCVD_OP_I3D_PREP ? "I3D_PREP" : "I3D_HEAD";
+      if (const char* why = op.kind == MCVD_OP_I3D_PREP ? i3d_prep_error(op) : i3d_head_error(op)) {
+        set_error("op %d %s: %s", idx, name, why);
         return -1;
       }
       if (misaligned(op.bias)) {
-        set_error("op %d %s: bias must be 16-byte aligned", idx, names[op.kind - MCVD_OP_I3D_PREP]);
+        set_error("op %d %s: bias must be 16-byte aligned", idx, name);
         return -1;
       }
       break;
@@ -186,31 +189,17 @@ static int validate_one(const McvdOp& op, int idx) {
       }
       break;
     case MCVD_OP_FID_PREP:
-    case MCVD_OP_CONV2D:
-    case MCVD_OP_MAXPOOL2D:
     case MCVD_OP_FID_HEAD:
     case MCVD_OP_KNN_RADIUS:
     case MCVD_OP_KNN_COVER: {
-      const char* why = op.kind == MCVD_OP_FID_PREP    ? fid_prep_error(op)
-                        : op.kind == MCVD_OP_CONV2D    ? conv2d_error(op)
-                        : op.kind == MCVD_OP_MAXPOOL2D ? maxpool2d_error(op)
-                        : op.kind == MCVD_OP_FID_HEAD  ? fid_head_error(op)
-                                                       : knn_error(op);
-      static const char* const names[] = {"FID_PREP", "CONV2D", "MAXPOOL2D", "FID_HEAD", "KNN_RADIUS", "KNN_COVER"};
+      const char* why = op.kind == MCVD_OP_FID_PREP   ? fid_prep_error(op)
+                        : op.kind == MCVD_OP_FID_HEAD ? fid_head_error(op)
+                                                      : knn_error(op);
+      const char* name = op.kind == MCVD_OP_FID_PREP     ? "FID_PREP"
+                         : op.kind == MCVD_OP_FID_HEAD   ? "FID_HEAD"
+                         : op.kind == MCVD_OP_KNN_RADIUS ? "KNN_RADIUS"
+                                                         : "KNN_COVER";
       if (why) {
-        set_error("op %d %s: %s", idx, names[op.kind - MCVD_OP_FID_PREP], why);
-        return -1;
-      }
-      if (misaligned(op.bias)) {
-        set_error("op %d %s: bias must be 16-byte aligned", idx, names[op.kind - MCVD_OP_FID_PREP]);
-        return -1;
-      }
-      break;
-    }
-    case MCVD_OP_CONV3D_TF32:
-    case MCVD_OP_CONV2D_TF32: {
-      const char* name = op.kind == MCVD_OP_CONV3D_TF32 ? "CONV3D_TF32" : "CONV2D_TF32";
-      if (const char* why = conv_tf32_error(op)) {
         set_error("op %d %s: %s", idx, name, why);
         return -1;
       }

@@ -1,6 +1,7 @@
 // TF32 tensor-core convolutions of the FVD (I3D) and FID (Inception-v3) feature networks: MCVD_OP_CONV3D_TF32 and
-// MCVD_OP_CONV2D_TF32 in include/mcvd_b200.h.  Same geometry, epilogue and channel-slice output as MCVD_OP_CONV3D
-// (i3d.cu) and MCVD_OP_CONV2D (inception.cu); the products run on wgmma m64nNk8 tf32 with fp32 accumulators.
+// MCVD_OP_CONV2D_TF32 in include/mcvd_b200.h.  Same geometry, gather, epilogue and channel-slice output as
+// MCVD_OP_CONV3D and MCVD_OP_CONV2D (conv_eval.cuh, conv_eval.cu); the products run on wgmma m64nNk8 tf32 with fp32
+// accumulators.
 //
 // Implicit GEMM: M = output positions (video * t * y * x, or frame * y * x), N = Cout, K = taps * Cin in
 // (dt, dy, dx, c) order.  A CTA of two warpgroups computes a 128-position x BN tile; K advances in slabs of 32.
@@ -13,9 +14,7 @@
 // The tensor cores therefore never see a value with low mantissa bits set, and nothing depends on how they treat
 // them.  Each output is one accumulator chain over K in slab order, with no split-K, so a video's or frame's
 // features are the same bits whichever M tile, chunk or batch position it lands in.
-#include <math.h>
-
-#include "mcvd_common.cuh"
+#include "conv_eval.cuh"
 #include "umma_ptx.cuh"
 
 namespace mcvd {
@@ -25,7 +24,6 @@ using namespace ptx;
 constexpr int TF_BM = 128;       // output positions per CTA: two consumer warpgroups of 64
 constexpr int TF_BK = 32;        // K per slab: 8 core-matrix columns of 4 tf32
 constexpr int TF_THREADS = 256;
-enum { TG_GENERAL = 0, TG_PW = 1, TG_MAXPOOL = 2, TG_AVGPOOL = 3 };
 
 // n tile for Cout: the width of {32, 64, 96, 128} with the smallest cost ntiles * (width + 64), where 64 stands for
 // the A operand each n tile re-gathers and re-stages; ties go to the wider tile.  Shared by packing and launch.
@@ -39,21 +37,6 @@ static int tf32_ntile(int Cout) {
   return best;
 }
 
-struct TfGeom {
-  int Tin, Sin, Cin, kt, kh, kw, st, ss, pt, ph, pw, To, Ho, Wo, Cout, K, pitch, off, nk, ntiles;
-  long long M;
-};
-
-struct TfPos {
-  const float* img;          // the position's video / frame (its input pixel for PW), NULL past the last position
-  int it0, iy0, ix0;         // front-top-left input coordinate of its window (the position itself for the pools)
-};
-
-struct TfTap {
-  int c, dt, dy, dx;
-  bool in;                   // k < K
-};
-
 __device__ __forceinline__ float tf32_rna(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -66,77 +49,6 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-template <int MODE>
-__device__ __forceinline__ TfPos tf_pos(const float* __restrict__ src, const TfGeom& g, long long m) {
-  TfPos q{nullptr, 0, 0, 0};
-  if (m >= g.M) return q;
-  if (MODE == TG_PW) {
-    q.img = src + m * g.Cin;
-    return q;
-  }
-  const int hw = g.Ho * g.Wo;
-  const int P = g.To * hw;
-  const long long n = m / P;
-  int r = (int)(m - n * P);
-  const int ot = r / hw;
-  r -= ot * hw;
-  const int oy = r / g.Wo;
-  q.img = src + n * g.Tin * g.Sin * g.Sin * g.Cin;
-  q.it0 = ot * g.st - g.pt;
-  q.iy0 = oy * g.ss - g.ph;
-  q.ix0 = (r - oy * g.Wo) * g.ss - g.pw;
-  return q;
-}
-
-template <int MODE>
-__device__ __forceinline__ TfTap tf_tap(const TfGeom& g, int k) {
-  TfTap t{k, 0, 0, 0, k < g.K};
-  if (MODE != TG_GENERAL || !t.in) return t;
-  const int tap = k / g.Cin;
-  t.c = k - tap * g.Cin;
-  const int khw = g.kh * g.kw;
-  t.dt = tap / khw;
-  const int r = tap - t.dt * khw;
-  t.dy = r / g.kw;
-  t.dx = r - t.dy * g.kw;
-  return t;
-}
-
-template <int MODE>
-__device__ __forceinline__ float4 tf_gather(const TfPos& q, const TfGeom& g, const TfTap& t) {
-  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (!q.img || !t.in) return zero;
-  if (MODE == TG_PW) return *reinterpret_cast<const float4*>(q.img + t.c);
-  if (MODE == TG_GENERAL) {
-    const int it = q.it0 + t.dt, iy = q.iy0 + t.dy, ix = q.ix0 + t.dx;
-    if (it < 0 || it >= g.Tin || iy < 0 || iy >= g.Sin || ix < 0 || ix >= g.Sin) return zero;
-    return *reinterpret_cast<const float4*>(q.img + (((long long)it * g.Sin + iy) * g.Sin + ix) * g.Cin + t.c);
-  }
-  // the 3x3 / stride-1 / pad-1 pool of the branch_pool convs, exactly as k_conv2d (inception.cu) forms it
-  const float init = MODE == TG_MAXPOOL ? -INFINITY : 0.f;
-  float4 v = make_float4(init, init, init, init);
-  int count = 0;
-#pragma unroll 1
-  for (int dy = -1; dy <= 1; ++dy)
-#pragma unroll 1
-    for (int dx = -1; dx <= 1; ++dx) {
-      const int iy = q.iy0 + dy, ix = q.ix0 + dx;
-      if (iy < 0 || iy >= g.Sin || ix < 0 || ix >= g.Sin) continue;
-      const float4 u = *reinterpret_cast<const float4*>(q.img + ((long long)iy * g.Sin + ix) * g.Cin + t.c);
-      if (MODE == TG_MAXPOOL) {
-        v.x = fmaxf(v.x, u.x); v.y = fmaxf(v.y, u.y); v.z = fmaxf(v.z, u.z); v.w = fmaxf(v.w, u.w);
-      } else {
-        v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w;
-        ++count;
-      }
-    }
-  if (MODE == TG_AVGPOOL) {
-    const float d = (float)count;
-    v.x /= d; v.y /= d; v.z /= d; v.w /= d;
-  }
-  return v;
-}
-
 // Shared memory: two stages of A [32 k / 4][128 rows][4] and B [32 k / 4][BN cols][4], both the K-major no-swizzle
 // core-matrix layout (8 rows x 16 bytes per core matrix, row groups 128 bytes apart, K columns of 4 a whole tile
 // apart).  Thread roles: in the gather, warp w stages rows 8w .. 8w+7 and 64 + 8w .. 64 + 8w+7, lane l row 8w + l % 8
@@ -146,27 +58,27 @@ __device__ __forceinline__ float4 tf_gather(const TfPos& q, const TfGeom& g, con
 template <int MODE, int BN>
 __global__ void __launch_bounds__(TF_THREADS, 2)
     k_conv_tf32(const float* __restrict__ src, const float* __restrict__ wp, const float* __restrict__ bias,
-                float* __restrict__ dst, TfGeom g) {
+                float* __restrict__ dst, ConvGeom g, int nk, int ntiles) {
   extern __shared__ __align__(128) float tf_smem[];
   constexpr int A_STAGE = TF_BM * TF_BK, B_STAGE = BN * TF_BK;    // floats
   float* As = tf_smem;
   float* Bs = tf_smem + 2 * A_STAGE;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nt = (int)(blockIdx.x % (unsigned)g.ntiles);
-  const long long m0 = (long long)(blockIdx.x / (unsigned)g.ntiles) * TF_BM;
+  const int nt = (int)(blockIdx.x % (unsigned)ntiles);
+  const long long m0 = (long long)(blockIdx.x / (unsigned)ntiles) * TF_BM;
   const int n0 = nt * BN;
   const int prow = 8 * warp + (lane & 7), pkc = lane >> 3;
-  const TfPos q[2] = {tf_pos<MODE>(src, g, m0 + prow), tf_pos<MODE>(src, g, m0 + prow + 64)};
-  const float* wtile = wp + (long long)nt * g.nk * B_STAGE;
+  const ConvPos q[2] = {conv_pos<MODE>(src, g, m0 + prow), conv_pos<MODE>(src, g, m0 + prow + 64)};
+  const float* wtile = wp + (long long)nt * nk * B_STAGE;
   const uint32_t as0 = smem_u32(As), bs0 = smem_u32(Bs);
 
   float4 ra[2][2];                                         // [K column j][row i] of the next slab
   auto load_a = [&](int kb) {
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
-      const TfTap t = tf_tap<MODE>(g, kb * TF_BK + 4 * (pkc + 4 * j));
+      const ConvTap t = conv_tap<MODE>(g, kb * TF_BK + 4 * (pkc + 4 * j));
 #pragma unroll
-      for (int i = 0; i < 2; ++i) ra[j][i] = tf_gather<MODE>(q[i], g, t);
+      for (int i = 0; i < 2; ++i) ra[j][i] = conv_gather<MODE, true>(q[i], g, t);
     }
   };
   auto store_a = [&](int s) {
@@ -200,9 +112,9 @@ __global__ void __launch_bounds__(TF_THREADS, 2)
 
   const int wg = warp >> 2;
   const uint64_t a_proto = make_desc(0, TF_BM * 16, 128), b_proto = make_desc(0, BN * 16, 128);
-  for (int kb = 0; kb < g.nk; ++kb) {
+  for (int kb = 0; kb < nk; ++kb) {
     const int s = kb & 1;
-    const bool more = kb + 1 < g.nk;
+    const bool more = kb + 1 < nk;
     if (more) {                                            // the next slab's loads fly while this slab's MMAs run
       load_a(kb + 1);
       load_b(kb + 1, s ^ 1);
@@ -266,32 +178,30 @@ static long long tf32_packed_floats(int K, int Cout) {
   return (long long)cdiv(K, TF_BK) * TF_BK * cdiv(Cout, bn) * bn;
 }
 
-// the geometry of either kind; the fp32 kind's checks, then the tile grid of this kernel
-const char* conv_tf32_error(const McvdOp& op) {
-  const bool three = op.kind == MCVD_OP_CONV3D_TF32;
-  if (const char* why = three ? conv3d_error(op) : conv2d_error(op)) return why;
-  const long long M = three ? (long long)op.B * same_out(op.i4, op.i0, op.i2) * op.H * op.W
-                            : (long long)op.B * op.H * op.W;
-  if ((M + TF_BM - 1) / TF_BM * cdiv(op.Cout, tf32_ntile(op.Cout)) > 0x7fffffffLL)
+const char* conv_tf32_geom(const McvdOp& op, ConvGeom& g) {
+  if (const char* why = conv_geom(op, g)) return why;
+  if ((g.M + TF_BM - 1) / TF_BM * cdiv(op.Cout, tf32_ntile(op.Cout)) > 0x7fffffffLL)
     return "too many output positions for the grid";
   return nullptr;
 }
 
 template <int MODE, int BN>
-static int run_tf32(const McvdOp& op, const TfGeom& g, cudaStream_t s) {
+static int run_tf32(const McvdOp& op, const ConvGeom& g, cudaStream_t s) {
   const size_t smem = (size_t)2 * (TF_BM + BN) * TF_BK * sizeof(float);
   cudaError_t e = cudaFuncSetAttribute(k_conv_tf32<MODE, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   MCVD_CHECK(e == cudaSuccess, "CONV_TF32: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-  const long long ctas = (g.M + TF_BM - 1) / TF_BM * g.ntiles;
+  const int ntiles = cdiv(g.Cout, BN);
+  const long long ctas = (g.M + TF_BM - 1) / TF_BM * ntiles;
   k_conv_tf32<MODE, BN><<<(unsigned)ctas, TF_THREADS, smem, s>>>((const float*)op.src0, (const float*)op.w,
-                                                                (const float*)op.bias, (float*)op.dst, g);
+                                                                (const float*)op.bias, (float*)op.dst, g,
+                                                                cdiv(g.K, TF_BK), ntiles);
   MCVD_CUDA_LAUNCH_CHECK("conv_tf32");
   return 0;
 }
 
 template <int MODE>
-static int run_tf32_mode(const McvdOp& op, const TfGeom& g, int bn, cudaStream_t s) {
-  switch (bn) {
+static int run_tf32_mode(const McvdOp& op, const ConvGeom& g, cudaStream_t s) {
+  switch (tf32_ntile(g.Cout)) {
     case 32: return run_tf32<MODE, 32>(op, g, s);
     case 64: return run_tf32<MODE, 64>(op, g, s);
     case 96: return run_tf32<MODE, 96>(op, g, s);
@@ -299,46 +209,16 @@ static int run_tf32_mode(const McvdOp& op, const TfGeom& g, int bn, cudaStream_t
   }
 }
 
-static int launch_tf32(const McvdOp& op, TfGeom& g, int mode, cudaStream_t s) {
-  const int bn = tf32_ntile(op.Cout);
-  g.Cout = op.Cout; g.pitch = op.i6; g.off = op.i7;
-  g.nk = cdiv(g.K, TF_BK);
-  g.ntiles = cdiv(op.Cout, bn);
-  switch (mode) {
-    case TG_PW: return run_tf32_mode<TG_PW>(op, g, bn, s);
-    case TG_MAXPOOL: return run_tf32_mode<TG_MAXPOOL>(op, g, bn, s);
-    case TG_AVGPOOL: return run_tf32_mode<TG_AVGPOOL>(op, g, bn, s);
-    default: return run_tf32_mode<TG_GENERAL>(op, g, bn, s);
+int launch_conv_tf32(const McvdOp& op, cudaStream_t s) {
+  ConvGeom g;
+  if (const char* why = conv_tf32_geom(op, g)) MCVD_CHECK(false, "%s: %s", conv_kind_name(op.kind), why);
+  switch (gather_mode(op)) {
+    case G_CONV2: return run_tf32_mode<G_CONV2>(op, g, s);
+    case G_CONV3: return run_tf32_mode<G_CONV3>(op, g, s);
+    case G_PW: return run_tf32_mode<G_PW>(op, g, s);
+    case G_BMAX: return run_tf32_mode<G_BMAX>(op, g, s);
+    default: return run_tf32_mode<G_BAVG>(op, g, s);
   }
-}
-
-int launch_conv3d_tf32(const McvdOp& op, cudaStream_t s) {
-  if (const char* why = conv_tf32_error(op)) MCVD_CHECK(false, "CONV3D_TF32: %s", why);
-  TfGeom g;
-  g.Tin = op.i4; g.Sin = op.i5; g.Cin = op.C0;
-  g.kt = op.i0; g.kh = g.kw = op.i1; g.st = op.i2; g.ss = op.i3;
-  g.pt = same_pad(op.i4, op.i0, op.i2) / 2;
-  g.ph = g.pw = same_pad(op.i5, op.i1, op.i3) / 2;
-  g.To = same_out(op.i4, op.i0, op.i2); g.Ho = g.Wo = op.H;
-  g.K = op.i0 * op.i1 * op.i1 * op.C0;
-  g.M = (long long)op.B * g.To * g.Ho * g.Wo;
-  const bool pw = op.i0 == 1 && op.i1 == 1 && op.i2 == 1 && op.i3 == 1;
-  return launch_tf32(op, g, pw ? TG_PW : TG_GENERAL, s);
-}
-
-int launch_conv2d_tf32(const McvdOp& op, cudaStream_t s) {
-  if (const char* why = conv_tf32_error(op)) MCVD_CHECK(false, "CONV2D_TF32: %s", why);
-  TfGeom g;
-  g.Tin = 1; g.Sin = op.i5; g.Cin = op.C0;
-  g.kt = 1; g.kh = op.i0; g.kw = op.i1; g.st = 1; g.ss = op.i2;
-  g.pt = 0; g.ph = op.i3; g.pw = op.i4;
-  g.To = 1; g.Ho = op.H; g.Wo = op.W;
-  g.K = op.i0 * op.i1 * op.C0;
-  g.M = (long long)op.B * op.H * op.W;
-  const int mode = (op.flags & MCVD_F_POOL) ? ((op.flags & MCVD_F_AVG) ? TG_AVGPOOL : TG_MAXPOOL)
-                   : (op.i0 == 1 && op.i1 == 1 && op.i2 == 1) ? TG_PW
-                                                              : TG_GENERAL;
-  return launch_tf32(op, g, mode, s);
 }
 
 }  // namespace mcvd

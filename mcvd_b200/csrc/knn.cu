@@ -3,7 +3,7 @@
 // of (a_d - b_d)^2 (one subtract and one FMA per term), so the same pair gives the same bits in every pass and a
 // point's distance to itself is exactly 0.
 //
-// Tiling (the FFMA tile of k_conv3d / k_conv2d): one CTA owns 64 rows of A and streams B past them in 64-row tiles,
+// Tiling (the FFMA tile of k_conv_ffma, conv_eval.cu): one CTA owns 64 rows of A and streams B past them in 64-row tiles,
 // 16 features deep, the next slice prefetched into registers; each thread holds a 4 x 4 block of squared distances.
 // After each B tile a thread folds its 16 distances into per-row state held in registers:
 //   RADIUS: the 8 smallest squared distances of each of its 4 rows over the columns it has seen (sorted, with

@@ -1,6 +1,6 @@
 // LPIPS v0.1 (net-lin, AlexNet backbone) of generated frames against real ones: see MCVD_OP_LPIPS_PREP,
 // MCVD_OP_CONV_RELU and MCVD_OP_LPIPS_LAYER in include/mcvd_b200.h.  One chunk of N frame pairs is 11 launches:
-// prep, then per AlexNet layer one convolution and one LPIPS head that consumes its tap.
+// prep, then per AlexNet layer one convolution (conv_eval.cu) and one LPIPS head that consumes its tap.
 #include "mcvd_common.cuh"
 
 namespace mcvd {
@@ -74,149 +74,6 @@ int launch_lpips_prep(const McvdOp& op, cudaStream_t s) {
   k_lpips_prep<<<grid, 256, 0, s>>>((const float*)op.src0, (const float*)op.src1, (const int*)op.w, (float*)op.dst,
                                     op.B * op.i0, op.C0, op.i0, op.i1, op.i2);
   MCVD_CUDA_LAUNCH_CHECK("lpips_prep");
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------------
-// NHWC direct convolution + bias + ReLU as an fp32 FFMA implicit GEMM: M = images * OH * OW output positions,
-// N = Cout, K = k * k * Cin in (ky, kx, c) order.  64 x 64 output tile per CTA, 16-deep K slices, 4 x 4 outputs
-// per thread, the next slice prefetched into registers while the current one is multiplied.  Every output is
-// accumulated by one thread in K order, so its value does not depend on the batch it is computed in.
-// POOL: the conv reads the 3x3/s2 max-pool of src (AlexNet features[2], [5]) instead of src itself.
-// ------------------------------------------------------------------------------------------------
-constexpr int CR_BM = 64, CR_BN = 64, CR_BK = 16;
-
-struct ConvGeom {
-  int Hin, Win, Hc, Wc, Cin, ks, stride, pad, OH, OW, Cout, K;
-  long long M;
-};
-
-// the output position one A-loader thread gathers for, decomposed once per CTA (not once per K slice)
-struct GatherPos {
-  const float* img;          // the position's image, NULL past the last position
-  int iy0, ix0;              // top-left input coordinate of its window
-};
-
-__device__ __forceinline__ GatherPos gather_pos(const float* __restrict__ src, const ConvGeom& g, long long m) {
-  GatherPos q{nullptr, 0, 0};
-  if (m >= g.M) return q;
-  const int P = g.OH * g.OW;
-  const long long n = m / P;
-  const int r = (int)(m - n * P);
-  q.img = src + n * g.Hin * g.Win * g.Cin;
-  q.iy0 = (r / g.OW) * g.stride - g.pad;
-  q.ix0 = (r % g.OW) * g.stride - g.pad;
-  return q;
-}
-
-template <bool POOL>
-__device__ __forceinline__ float4 conv_gather(const GatherPos& q, const ConvGeom& g, int k) {
-  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (!q.img || k >= g.K) return zero;
-  const int tap = k / g.Cin, c = k - tap * g.Cin;
-  const int ky = tap / g.ks;
-  const int iy = q.iy0 + ky, ix = q.ix0 + tap - ky * g.ks;
-  if (iy < 0 || iy >= g.Hc || ix < 0 || ix >= g.Wc) return zero;
-  const float* img = q.img + c;
-  if (!POOL) return *reinterpret_cast<const float4*>(img + ((long long)iy * g.Win + ix) * g.Cin);
-  float4 v = *reinterpret_cast<const float4*>(img + ((long long)(2 * iy) * g.Win + 2 * ix) * g.Cin);
-#pragma unroll
-  for (int dy = 0; dy < 3; ++dy)
-#pragma unroll
-    for (int dx = 0; dx < 3; ++dx) {
-      if (dy == 0 && dx == 0) continue;
-      const float4 u = *reinterpret_cast<const float4*>(img + ((long long)(2 * iy + dy) * g.Win + 2 * ix + dx) * g.Cin);
-      v.x = fmaxf(v.x, u.x); v.y = fmaxf(v.y, u.y); v.z = fmaxf(v.z, u.z); v.w = fmaxf(v.w, u.w);
-    }
-  return v;
-}
-
-template <bool POOL>
-__global__ void __launch_bounds__(256) k_conv_relu(const float* __restrict__ src, const float* __restrict__ w,
-                                                   const float* __restrict__ bias, float* __restrict__ dst, ConvGeom g) {
-  __shared__ __align__(16) float As[2][CR_BK][CR_BM];
-  __shared__ __align__(16) float Bs[2][CR_BK][CR_BN];
-  const int tid = threadIdx.x;
-  const long long m0 = (long long)blockIdx.x * CR_BM;
-  const int n0 = blockIdx.y * CR_BN;
-  // loader roles: A = one position x 4 consecutive k (4 channels of one tap); B = one k row x 4 output channels
-  const int am = tid % CR_BM, ak = (tid / CR_BM) * 4;
-  const int bk = tid / (CR_BN / 4), bn = (tid % (CR_BN / 4)) * 4;
-  const int tm = (tid / 16) * 4, tn = (tid % 16) * 4;
-  float acc[4][4] = {};
-  const GatherPos q = gather_pos(src, g, m0 + am);
-  float4 ra = conv_gather<POOL>(q, g, ak);
-  float4 rb = bk < g.K ? *reinterpret_cast<const float4*>(w + (long long)bk * g.Cout + n0 + bn)
-                       : make_float4(0.f, 0.f, 0.f, 0.f);
-  int buf = 0;
-  for (int k0 = 0; k0 < g.K; k0 += CR_BK) {
-    As[buf][ak + 0][am] = ra.x; As[buf][ak + 1][am] = ra.y; As[buf][ak + 2][am] = ra.z; As[buf][ak + 3][am] = ra.w;
-    *reinterpret_cast<float4*>(&Bs[buf][bk][bn]) = rb;
-    __syncthreads();
-    const int k1 = k0 + CR_BK;
-    if (k1 < g.K) {
-      ra = conv_gather<POOL>(q, g, k1 + ak);
-      rb = k1 + bk < g.K ? *reinterpret_cast<const float4*>(w + (long long)(k1 + bk) * g.Cout + n0 + bn)
-                         : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-#pragma unroll
-    for (int kk = 0; kk < CR_BK; ++kk) {
-      const float4 a = *reinterpret_cast<const float4*>(&As[buf][kk][tm]);
-      const float4 b = *reinterpret_cast<const float4*>(&Bs[buf][kk][tn]);
-      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-    }
-    buf ^= 1;                                      // the other buffer was last read before this slice's barrier
-  }
-  const float4 bb = *reinterpret_cast<const float4*>(bias + n0 + tn);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const long long m = m0 + tm + i;
-    if (m >= g.M) break;
-    float4 o;
-    o.x = fmaxf(acc[i][0] + bb.x, 0.f);
-    o.y = fmaxf(acc[i][1] + bb.y, 0.f);
-    o.z = fmaxf(acc[i][2] + bb.z, 0.f);
-    o.w = fmaxf(acc[i][3] + bb.w, 0.f);
-    *reinterpret_cast<float4*>(dst + m * g.Cout + n0 + tn) = o;
-  }
-}
-
-// NULL, or why the geometry of a MCVD_OP_CONV_RELU op is unusable (shared by validation and launch)
-const char* conv_relu_error(const McvdOp& op) {
-  if (!op.w || !op.bias) return "null weights or bias";
-  if (op.C0 <= 0 || op.C0 % 4) return "input channels must be a positive multiple of 4";
-  if (op.Cout <= 0 || op.Cout % CR_BN) return "output channels must be a positive multiple of 64";
-  if (op.i0 < 1 || op.i1 < 1 || op.i2 < 0) return "kernel size, stride or padding out of range";
-  if (op.i3 < 1 || op.i4 < 1) return "input size out of range";
-  const bool pool = (op.flags & MCVD_F_POOL) != 0;
-  if (pool && (op.i3 < 3 || op.i4 < 3)) return "pooled input smaller than the 3x3 window";
-  const int hc = pool ? (op.i3 - 3) / 2 + 1 : op.i3, wc = pool ? (op.i4 - 3) / 2 + 1 : op.i4;
-  if (hc + 2 * op.i2 < op.i0 || wc + 2 * op.i2 < op.i0) return "kernel larger than the padded input";
-  if (op.H != (hc + 2 * op.i2 - op.i0) / op.i1 + 1 || op.W != (wc + 2 * op.i2 - op.i0) / op.i1 + 1)
-    return "output size disagrees with the convolution geometry";
-  return nullptr;
-}
-
-int launch_conv_relu(const McvdOp& op, cudaStream_t s) {
-  MCVD_CHECK(op.src0 && op.dst, "CONV_RELU: null pointer");
-  if (const char* why = conv_relu_error(op)) MCVD_CHECK(false, "CONV_RELU: %s", why);
-  const bool pool = (op.flags & MCVD_F_POOL) != 0;
-  ConvGeom g;
-  g.Hin = op.i3; g.Win = op.i4; g.Cin = op.C0; g.ks = op.i0; g.stride = op.i1; g.pad = op.i2;
-  g.Hc = pool ? (op.i3 - 3) / 2 + 1 : op.i3;
-  g.Wc = pool ? (op.i4 - 3) / 2 + 1 : op.i4;
-  g.OH = op.H; g.OW = op.W; g.Cout = op.Cout; g.K = op.i0 * op.i0 * op.C0;
-  g.M = (long long)op.B * op.H * op.W;
-  dim3 grid((unsigned)((g.M + CR_BM - 1) / CR_BM), op.Cout / CR_BN);
-  if (pool) k_conv_relu<true><<<grid, 256, 0, s>>>((const float*)op.src0, (const float*)op.w, (const float*)op.bias,
-                                                   (float*)op.dst, g);
-  else k_conv_relu<false><<<grid, 256, 0, s>>>((const float*)op.src0, (const float*)op.w, (const float*)op.bias,
-                                               (float*)op.dst, g);
-  MCVD_CUDA_LAUNCH_CHECK("conv_relu");
   return 0;
 }
 

@@ -62,44 +62,30 @@ int launch_attention_umma(const McvdOp& op, cudaStream_t s);
 int launch_frame_metrics(const McvdOp& op, cudaStream_t s);
 int launch_noise(const McvdOp& op, cudaStream_t s);
 int launch_lpips_prep(const McvdOp& op, cudaStream_t s);
-int launch_conv_relu(const McvdOp& op, cudaStream_t s);
 int launch_lpips_layer(const McvdOp& op, cudaStream_t s);
 int launch_i3d_prep(const McvdOp& op, cudaStream_t s);
-int launch_conv3d(const McvdOp& op, cudaStream_t s);
-int launch_maxpool3d(const McvdOp& op, cudaStream_t s);
 int launch_i3d_head(const McvdOp& op, cudaStream_t s);
 int launch_dsm_perturb(const McvdOp& op, cudaStream_t s);
 int launch_dsm_loss(const McvdOp& op, cudaStream_t s);
 int launch_fid_prep(const McvdOp& op, cudaStream_t s);
-int launch_conv2d(const McvdOp& op, cudaStream_t s);
-int launch_maxpool2d(const McvdOp& op, cudaStream_t s);
 int launch_fid_head(const McvdOp& op, cudaStream_t s);
 int launch_knn(const McvdOp& op, cudaStream_t s);
-
-// NULL, or why the geometry of a MCVD_OP_CONV_RELU op is unusable
-const char* conv_relu_error(const McvdOp& op);
+int launch_conv_ffma(const McvdOp& op, cudaStream_t s);   // CONV_RELU, CONV3D, CONV2D (conv_eval.cu)
+int launch_maxpool(const McvdOp& op, cudaStream_t s);     // MAXPOOL3D, MAXPOOL2D (conv_eval.cu)
+int launch_conv_tf32(const McvdOp& op, cudaStream_t s);   // CONV3D_TF32, CONV2D_TF32 (conv_tf32.cu)
 
 // NULL, or why an op of the I3D kinds is unusable (shared by validation and launch; i3d.cu)
 const char* i3d_prep_error(const McvdOp& op);
-const char* conv3d_error(const McvdOp& op);
-const char* maxpool3d_error(const McvdOp& op);
 const char* i3d_head_error(const McvdOp& op);
 
 // NULL, or why a MCVD_OP_DSM_PERTURB / MCVD_OP_DSM_LOSS op is unusable (shared by validation and launch; dsm.cu)
 const char* dsm_error(const McvdOp& op);
 
-// NULL, or why an op of the FID kinds is unusable (shared by validation and launch; inception.cu, knn.cu)
+// NULL, or why an op of the FID kinds is unusable (shared by validation and launch; inception.cu, knn.cu).  The conv
+// and max-pool kinds of LPIPS, I3D and Inception-v3 are validated by conv_geom / conv_tf32_geom (conv_eval.cuh).
 const char* fid_prep_error(const McvdOp& op);
-const char* conv2d_error(const McvdOp& op);
-const char* maxpool2d_error(const McvdOp& op);
 const char* fid_head_error(const McvdOp& op);
 const char* knn_error(const McvdOp& op);
-
-// MCVD_OP_CONV3D_TF32 / MCVD_OP_CONV2D_TF32 (conv_tf32.cu): NULL, or why the op is unusable (shared by validation and
-// launch), and the launchers
-const char* conv_tf32_error(const McvdOp& op);
-int launch_conv3d_tf32(const McvdOp& op, cudaStream_t s);
-int launch_conv2d_tf32(const McvdOp& op, cudaStream_t s);
 
 // NULL, or why the Gamma parameters (f6 = shape, f7 = scale) of an op with MCVD_F_GAMMA are unusable
 const char* gamma_params_error(const McvdOp& op);

@@ -28,10 +28,12 @@ from __future__ import annotations
 
 import functools
 import os
-from typing import Dict, List, Optional, Union
+from typing import List, Optional, Union
 
 import numpy as np
 import torch
+
+from . import eval_weights as EW
 
 SIDE = 299                         # InceptionV3.forward resizes to 299x299 (evaluation/inception.py:146-150)
 DIMS = 2048
@@ -221,25 +223,6 @@ LAUNCHES_PER_CHUNK = len(plan()[0])
 DEFAULT_CHUNK = WORKSPACE_BUDGET // (4 * workspace_floats())
 
 
-def _load(obj) -> Dict[str, torch.Tensor]:
-    if isinstance(obj, dict):
-        return obj
-    try:
-        return torch.load(obj, map_location="cpu", weights_only=True)
-    except Exception as e:                          # noqa: BLE001 -- any unreadable file is a bad weight file
-        raise ValueError(f"InceptionV3: cannot read the Inception weights from {obj!r}: {e}") from e
-
-
-def _get(sd: Dict[str, torch.Tensor], key: str, shape) -> torch.Tensor:
-    if key not in sd:
-        raise ValueError(f"InceptionV3: weight {key!r} missing")
-    t = sd[key]
-    if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(shape):
-        got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
-        raise ValueError(f"InceptionV3: weight {key!r} has shape {got}, expected {tuple(shape)}")
-    return t.detach().cpu().double()
-
-
 def _prefix(sd, key: str) -> str:
     """The state_dict prefix of unit ``key`` (torchvision name): itself, or its ``blocks.*`` name in the reference
     wrapper's layout."""
@@ -249,29 +232,13 @@ def _prefix(sd, key: str) -> str:
     return BLOCK_PREFIX[top] + ("." + rest if rest else "")
 
 
-def fold_unit(sd, key: str, cin: int, cout: int, k) -> tuple:
-    """(w [kh*kw*Cin4, Cout], bias [Cout]) fp32 of one BasicConv2d, in the layout ``MCVD_OP_CONV2D`` reads:
-    BatchNorm2d (eps 1e-3, running statistics) folded into the convolution in fp64 and rounded once; Cin padded to
-    a multiple of 4 with zero weights."""
-    p = _prefix(sd, key)
-    kh, kw = k
-    w = _get(sd, p + ".conv.weight", (cout, cin, kh, kw))
-    gamma = _get(sd, p + ".bn.weight", (cout,))
-    beta = _get(sd, p + ".bn.bias", (cout,))
-    mean = _get(sd, p + ".bn.running_mean", (cout,))
-    var = _get(sd, p + ".bn.running_var", (cout,))
-    scale = gamma / torch.sqrt(var + BN_EPS)
-    cin4 = -(-cin // 4) * 4
-    packed = torch.zeros(kh, kw, cin4, cout, dtype=torch.float64)
-    packed[:, :, :cin, :] = (w * scale[:, None, None, None]).permute(2, 3, 1, 0)
-    return packed.reshape(kh * kw * cin4, cout).float().contiguous(), (beta - mean * scale).float().contiguous()
-
-
 def pack_weights(state_dict_or_path) -> dict:
-    """{unit key: (w, bias)} fp32 on the CPU for the 94 BasicConv2d.  Raises ``ValueError`` naming the first
+    """{unit key: (w, bias)} fp32 on the CPU for the 94 BasicConv2d, in the layout ``MCVD_OP_CONV2D`` reads, with
+    their BatchNorm2d (eps 1e-3) folded in (``eval_weights.fold_bn``).  Raises ``ValueError`` naming the first
     missing or misshapen key."""
-    sd = _load(state_dict_or_path)
-    return {key: fold_unit(sd, key, cin, cout, k) for key, cin, cout, k in units()}
+    sd = EW.load(state_dict_or_path, "InceptionV3", "Inception")
+    return {key: EW.fold_bn(sd, "InceptionV3", _prefix(sd, key), ".conv.weight", (cout, cin, *k), BN_EPS)
+            for key, cin, cout, k in units()}
 
 
 class InceptionV3:

@@ -27,6 +27,8 @@ from typing import Dict, List, Optional, Union
 import numpy as np
 import torch
 
+from . import eval_weights as EW
+
 SIDE = 224                         # preprocess_single(resolution=224)
 MIN_FRAMES = 9                     # at 8 frames the last time extent is 1, too short for the [2, 7, 7] average pool
 FVD_MIN_FRAMES = 10                # video_gen computes a task's FVD only for videos of at least 10 frames (:1311-1332)
@@ -87,48 +89,15 @@ def resize_target(S: int):
     return math.ceil(S * scale), SIDE
 
 
-def _load(obj) -> Dict[str, torch.Tensor]:
-    if isinstance(obj, dict):
-        return obj
-    try:
-        return torch.load(obj, map_location="cpu", weights_only=True)
-    except Exception as e:                          # noqa: BLE001 -- any unreadable file is a bad weight file
-        raise ValueError(f"I3D: cannot read the InceptionI3d weights from {obj!r}: {e}") from e
-
-
-def _get(sd: Dict[str, torch.Tensor], key: str, shape) -> torch.Tensor:
-    if key not in sd:
-        raise ValueError(f"I3D: weight {key!r} missing")
-    t = sd[key]
-    if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(shape):
-        got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
-        raise ValueError(f"I3D: weight {key!r} has shape {got}, expected {tuple(shape)}")
-    return t.detach().cpu().double()
-
-
-def fold_unit(sd, key: str, cin: int, cout: int, k: int):
-    """(w [k*k*k*Cin4, Cout], bias [Cout]) fp32 of one Unit3D, in the layout ``MCVD_OP_CONV3D`` reads: BatchNorm3d
-    (eps 1e-5, running statistics) folded into the convolution in fp64 and rounded once; Cin padded to a multiple
-    of 4 with zero weights."""
-    w = _get(sd, key + ".conv3d.weight", (cout, cin, k, k, k))
-    gamma = _get(sd, key + ".bn.weight", (cout,))
-    beta = _get(sd, key + ".bn.bias", (cout,))
-    mean = _get(sd, key + ".bn.running_mean", (cout,))
-    var = _get(sd, key + ".bn.running_var", (cout,))
-    scale = gamma / torch.sqrt(var + BN_EPS)
-    cin4 = -(-cin // 4) * 4
-    packed = torch.zeros(k, k, k, cin4, cout, dtype=torch.float64)
-    packed[..., :cin, :] = (w * scale[:, None, None, None, None]).permute(2, 3, 4, 1, 0)
-    return packed.reshape(k * k * k * cin4, cout).float().contiguous(), (beta - mean * scale).float().contiguous()
-
-
 def pack_weights(state_dict_or_path) -> dict:
     """{unit key: (w, bias)} for the 57 Unit3D plus ``"logits"``: (w [1024, 400], bias [400]) fp32 on the CPU.
-    Raises ``ValueError`` naming the first missing or misshapen key."""
-    sd = _load(state_dict_or_path)
-    packed = {key: fold_unit(sd, key, cin, cout, k) for key, cin, cout, k in units()}
-    w = _get(sd, "logits.conv3d.weight", (NUM_CLASSES, HEAD_CHANNELS, 1, 1, 1))
-    b = _get(sd, "logits.conv3d.bias", (NUM_CLASSES,))
+    A Unit3D's (w, bias) is in the layout ``MCVD_OP_CONV3D`` reads, with its BatchNorm3d (eps 1e-5) folded in
+    (``eval_weights.fold_bn``).  Raises ``ValueError`` naming the first missing or misshapen key."""
+    sd = EW.load(state_dict_or_path, "I3D", "InceptionI3d")
+    packed = {key: EW.fold_bn(sd, "I3D", key, ".conv3d.weight", (cout, cin, k, k, k), BN_EPS)
+              for key, cin, cout, k in units()}
+    w = EW.get(sd, "logits.conv3d.weight", (NUM_CLASSES, HEAD_CHANNELS, 1, 1, 1), "I3D", torch.float64)
+    b = EW.get(sd, "logits.conv3d.bias", (NUM_CLASSES,), "I3D", torch.float64)
     packed["logits"] = (w.reshape(NUM_CLASSES, HEAD_CHANNELS).t().float().contiguous(), b.float().contiguous())
     return packed
 

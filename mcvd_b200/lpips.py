@@ -21,6 +21,8 @@ from typing import Dict, List, Optional, Union
 import numpy as np
 import torch
 
+from . import eval_weights as EW
+
 SIDE = 128                         # Resize((128, 128)) of the reference's T2 transform
 _PREC = 22                         # Pillow's PRECISION_BITS for 8-bit images
 
@@ -54,30 +56,11 @@ def pil_bilinear_table(size: int, out: int = SIDE) -> np.ndarray:
     return table
 
 
-def _load(obj, what: str) -> Dict[str, torch.Tensor]:
-    if isinstance(obj, dict):
-        return obj
-    try:
-        return torch.load(obj, map_location="cpu", weights_only=True)
-    except Exception as e:                          # noqa: BLE001 -- any unreadable file is a bad weight file
-        raise ValueError(f"LPIPS: cannot read the {what} weights from {obj!r}: {e}") from e
-
-
-def _get(sd: Dict[str, torch.Tensor], key: str, shape) -> torch.Tensor:
-    if key not in sd:
-        raise ValueError(f"LPIPS: weight {key!r} missing")
-    t = sd[key]
-    if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(shape):
-        got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
-        raise ValueError(f"LPIPS: weight {key!r} has shape {got}, expected {tuple(shape)}")
-    return t.detach().float().cpu()
-
-
 def pack_weights(backbone, lin=None) -> List[tuple]:
     """[(w [k*k*Cin4, Cout], bias [Cout], lin [Cout])] per AlexNet layer, fp32 on the CPU, in the layout
     ``MCVD_OP_CONV_RELU`` reads (Cin padded to a multiple of 4 with zero weights).  Raises ``ValueError`` naming
     the first missing or misshapen key."""
-    sd = _load(backbone, "backbone")
+    sd = EW.load(backbone, "LPIPS", "backbone")
     pnet = any(k.startswith("net.slice") for k in sd)
     if pnet:
         if lin is not None:
@@ -86,17 +69,14 @@ def pack_weights(backbone, lin=None) -> List[tuple]:
     else:
         if lin is None:
             raise ValueError("LPIPS: a torchvision AlexNet state_dict needs the LPIPS lin weights (alex.pth)")
-        lsd = _load(lin, "lin")
+        lsd = EW.load(lin, "LPIPS", "lin")
     packed = []
     for li, (idx, cin, cout, k, _, _, _) in enumerate(LAYERS):
         pre = f"net.slice{_PNET_SLICE[idx]}.{idx}." if pnet else f"features.{idx}."
-        w = _get(sd, pre + "weight", (cout, cin, k, k))
-        b = _get(sd, pre + "bias", (cout,))
-        lw = _get(lsd, f"lin{li}.model.1.weight", (1, cout, 1, 1)).reshape(cout)
-        cin4 = -(-cin // 4) * 4
-        wt = torch.zeros(k, k, cin4, cout)
-        wt[:, :, :cin] = w.permute(2, 3, 1, 0)
-        packed.append((wt.reshape(k * k * cin4, cout).contiguous(), b.contiguous(), lw.contiguous()))
+        w = EW.get(sd, pre + "weight", (cout, cin, k, k), "LPIPS", torch.float32)
+        b = EW.get(sd, pre + "bias", (cout,), "LPIPS", torch.float32)
+        lw = EW.get(lsd, f"lin{li}.model.1.weight", (1, cout, 1, 1), "LPIPS", torch.float32).reshape(cout)
+        packed.append((EW.kmajor(w), b.contiguous(), lw.contiguous()))
     return packed
 
 
