@@ -109,7 +109,9 @@ enum {
    * where 192 would leave SMs idle; else 128), 128 or 192 = forced (192 is an error where it cannot run); i5 = slab
    * stages of a streaming conv, a diagnostic override of the same kind: 0 = the launcher's choice (2), 2 or 3 =
    * forced (an error where it does not fit or the conv is input-stationary); i3 = operand split for accuracy experiments (0 | 3 = all three products, 1 = drop
-   * hi*lo_w, 2 = drop lo_a*hi, 4 = hi*hi only); f1 = weight un-scale.  Optional second K-segment (src2|src3 with C2|C3 channels, RAW,
+   * hi*lo_w, 2 = drop lo_a*hi, 4 = hi*hi only); f1 = weight un-scale.  MCVD_F_HALF: half mode, one fp16 product
+   * hi*hi per step (the 11-bit significand of TF32) instead of the hi/lo split; w must then be the hi-only image
+   * (mcvd_umma_pack_weights_ex with parts = 1) and i3 must be 0 or 3.  Optional second K-segment (src2|src3 with C2|C3 channels, RAW,
    * centre tap only, weights appended per n-tile): the 1x1 shortcut Conv_2(x) of ResnetBlockBigGANpp
    * (layerspp.py:618-619) accumulated into the same accumulators as Conv_1, so
    * dst = f0 * (Conv_1(act(norm(h))) + Conv_2(x) + bias + residual) in ONE kernel.
@@ -137,6 +139,7 @@ enum {
    *          (i2 = mcvd_umma2_plan(...); 0 skips the consistency check);
    *   i3   = operand split: 3 (default, also 0) = hi*hi + lo*hi + hi*lo, 1 = drop hi*lo (fp16 weights),
    *          2 = drop lo*hi (fp16 activations), 4 = hi*hi only -- accuracy experiments;
+   *   MCVD_F_HALF as for MCVD_OP_CONV_UMMA;
    *   dst2 = NULL, or int64 [tiles][NJ][2][Cout] receiving the GroupNorm partial sums of the stored output
    *          (sum and sum of squares of round(x * 2^16), exact integer arithmetic for |x| <= 2^12: round(x * 2^16)
    *          stays inside int32 and the sum of squares of a tile slot's 128 rows inside 64 bits; outputs beyond
@@ -284,6 +287,7 @@ enum {
                                       CONV2D: 3x3 / stride-1 / pad-1 max-pool on the input read     */
 #define MCVD_F_L1       (1 << 10)  /* DSM_LOSS: sum |z - eps| instead of 0.5 (z - eps)^2               */
 #define MCVD_F_AVG      (1 << 11)  /* CONV2D (with POOL): average pool, count_include_pad=False        */
+#define MCVD_F_HALF     (1 << 12)  /* CONV_UMMA, CONV_UMMA2: one fp16 product (hi-only weight image)  */
 
 typedef struct McvdOp {
   int32_t kind;
@@ -337,6 +341,12 @@ int mcvd_count_launches(const McvdOp* ops, int n);
  * scale_log2 receives the power-of-two pre-scale applied to the weights (undone in the epilogue). */
 long long mcvd_umma_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int k_block,
                                  void* out, int scale_log2, void* stream);
+/* mcvd_umma_pack_weights with every parameter: stage_off / per_unit place the image in a larger one as
+ * mcvd_umma2_pack_weights does (0 and (Cin / k_block) * taps for a stand-alone image), and parts selects the image:
+ * 2 = fp16 hi + lo (the default mode, taps*Cin*Cout*4 bytes), 1 = hi only (MCVD_F_HALF ops, taps*Cin*Cout*2 bytes,
+ * the same hi values).  Returns the bytes this call fills; out == NULL only queries. */
+long long mcvd_umma_pack_weights_ex(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int k_block,
+                                    void* out, int scale_log2, int stage_off, int per_unit, int parts, void* stream);
 /* Channels per K-block (32, 16, or 0 = unsupported) the tensor-core conv uses for sources with C0 / C1
  * channels; the packed weights must be produced with the same value. */
 int mcvd_umma_kblock(int C0, int C1);

@@ -51,6 +51,19 @@ class NetSpec:
     film_total: int                # total FiLM outputs (sum of 2*ch over every act-norm with an embedding)
 
 
+CONV_PRECISIONS = ("fp32", "fp16")
+
+
+def conv_precision(config) -> str:
+    """``config.model.conv_precision``: "fp32" (default, also when the key is missing) runs every tensor-core conv
+    with fp32 parity; "fp16" runs the convs that lower the reference's nn.Conv2d layers with one fp16 product, the
+    11-bit significand of the TF32 convolutions cuDNN runs for the reference.  Anything else is an error."""
+    p = getattr(config.model, "conv_precision", "fp32")
+    if p not in CONV_PRECISIONS:
+        raise ValueError(f"model.conv_precision must be 'fp32' or 'fp16', got {p!r}")
+    return p
+
+
 def check_supported(config) -> Optional[str]:
     """Return None if the fast path covers this config, else the reason it does not."""
     m, d = config.model, config.data

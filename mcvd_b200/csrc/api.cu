@@ -100,6 +100,10 @@ static int validate_one(const McvdOp& op, int idx) {
         set_error("op %d CONV: null weights or kernel size %d", idx, op.i0);
         return -1;
       }
+      if (op.kind != MCVD_OP_CONV_SIMT && (op.flags & MCVD_F_HALF) && op.i3 != 0 && op.i3 != 3) {
+        set_error("op %d CONV: MCVD_F_HALF runs one product; operand split %d must be 0 or 3", idx, op.i3);
+        return -1;
+      }
       break;
     case MCVD_OP_ATTENTION:
     case MCVD_OP_ATTENTION_UMMA:

@@ -11,6 +11,11 @@
 // lo*lo term and the second-level rounding are ~2^-22 relative.  Weights are pre-scaled by a power of
 // two (undone in the epilogue) so their lo parts stay in the fp16 normal range.
 //
+// Half mode (MCVD_F_HALF, template HALF): one product  hi*hi  per (tap, k16 step), the 11-bit significand of the
+// TF32 convolutions cuDNN runs for the reference.  Only hi is converted and staged (a slab stage is one half image)
+// and only hi is packed and streamed (a weight k16 step is 32 * NT bytes); everything else -- norm / FiLM / SiLU,
+// raw TMA stages, work organisation, the epilogue -- is the same code.
+//
 // "Padded-flat" implicit GEMM.  The batch is viewed as one flat array of positions
 //     q = b*(H+1)*(W+1) + r*(W+1) + c,   r in [0,H], c in [0,W],   pixel (y,x) = (r-1, c-1)
 // where row r = 0 and column c = 0 are zero padding shared between neighbouring rows / images.  In
@@ -141,7 +146,7 @@ __device__ __forceinline__ int first_raw(const ConvArgs& a, int q) {
   return (b * a.H + (rr - 1)) * a.W + (cc == 0 ? 0 : cc - 1);
 }
 
-template <int NT, int NWG>
+template <int NT, int NWG, bool HALF>
 __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs a,
                                                                   const __grid_constant__ ConvMaps maps) {
   static_assert(NWG == 2 || (NWG == 3 && NT <= NT_MAX3), "three consumer warpgroups hold at most 96 accumulators");
@@ -151,8 +156,8 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int chunks = a.KB / 8;
   const uint32_t a_half_bytes = (uint32_t)chunks * a.HP * 16;       // one of hi / lo
-  const uint32_t a_stage_bytes = 2 * a_half_bytes;
-  constexpr uint32_t b_step_bytes = 64u * NT;                        // one k16 step: hi (2 chunks) + lo
+  const uint32_t a_stage_bytes = HALF ? a_half_bytes : 2 * a_half_bytes;
+  constexpr uint32_t b_step_bytes = (HALF ? 32u : 64u) * NT;         // one k16 step: hi (2 chunks) [+ lo]
   const uint32_t b_stage_bytes = (uint32_t)(a.KB / 16) * b_step_bytes;
   uint8_t* a_base = smem_raw;
   uint8_t* b_base = a_base + (size_t)a.SA * a_stage_bytes;
@@ -322,13 +327,18 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
                 if (a.act_in) silu_fast8(v);
               }
               uint32_t hw[4], lw[4];
+              if constexpr (HALF) {
 #pragma unroll
-              for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
+                for (int e = 0; e < 4; ++e) hw[e] = cvt_hi2(v[2 * e], v[2 * e + 1]);
+              } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
+                lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+              }
               hv = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-              lv = make_uint4(lw[0], lw[1], lw[2], lw[3]);
             }
             *reinterpret_cast<uint4*>(hi_base + (size_t)h * 16) = hv;
-            *reinterpret_cast<uint4*>(lo_base + (size_t)h * 16) = lv;
+            if constexpr (!HALF) *reinterpret_cast<uint4*>(lo_base + (size_t)h * 16) = lv;
           }
           fence_proxy_async();          // make the generic-proxy stores visible to the tensor-core (async) proxy
           mbar_arrive(A_FULL(st));
@@ -392,12 +402,14 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
 #pragma unroll 1
           for (int s = 0; s < ksteps; ++s) {
             const uint64_t dbh = desc_add(b_proto, b_tap16 + (uint32_t)s * (b_step_bytes >> 4));
-            const uint64_t dbl = desc_add(dbh, b_lo16);
             const uint64_t dah = desc_add(a_proto, a_tap16 + (uint32_t)(2 * s) * a_lbo16);
-            const uint64_t dal = desc_add(dah, a_half16);
             wgmma_ss<NT>(acc, dah, dbh, 1);
-            if (a.split & 1) wgmma_ss<NT>(acc, dal, dbh, 1);
-            if (a.split & 2) wgmma_ss<NT>(acc, dah, dbl, 1);
+            if constexpr (!HALF) {
+              const uint64_t dbl = desc_add(dbh, b_lo16);
+              const uint64_t dal = desc_add(dah, a_half16);
+              if (a.split & 1) wgmma_ss<NT>(acc, dal, dbh, 1);
+              if (a.split & 2) wgmma_ss<NT>(acc, dah, dbl, 1);
+            }
           }
           wgmma_commit();
           wgmma_wait<1>();                                 // the previous group is complete: release its stages
@@ -493,10 +505,11 @@ __global__ void __launch_bounds__(128 * (NWG + 1), 1) k_conv_umma(const ConvArgs
 
 // ---- weight packing ---------------------------------------------------------------------------------
 // in : w_taps fp32 [taps][Cin][Cout]
-// out: fp16 stages of (KB/16) k16 steps, each  hi[2 chunks][NT][8]  then  lo[2 chunks][NT][8]; stage of
-//      (n tile nt, K-block kb, tap) = nt * per_unit + stage_off + kb * taps + tap
+// out: fp16 stages of (KB/16) k16 steps, each  hi[2 chunks][NT][8]  then (parts = 2)  lo[2 chunks][NT][8]; stage of
+//      (n tile nt, K-block kb, tap) = nt * per_unit + stage_off + kb * taps + tap.  parts = 1 is the half-mode image:
+//      the same hi values, half the bytes.
 __global__ void k_pack_weights(const float* __restrict__ w, __half* __restrict__ out, int taps, int Cin, int Cout,
-                               int NT, int KB, float scale, int stage_off, int per_unit) {
+                               int NT, int KB, float scale, int stage_off, int per_unit, int parts) {
   const int ksteps = KB / 16, nKB = Cin / KB, nNT = Cout / NT;
   const long long total = (long long)nNT * nKB * taps * ksteps * 2 * NT * 8;  // (chunk j, n, e) per step
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -514,10 +527,10 @@ __global__ void k_pack_weights(const float* __restrict__ w, __half* __restrict__
     __half h = __float2half_rn(v);
     __half l = __float2half_rn(v - __half2float(h));
     long long step = ((long long)nt * per_unit + stage_off + (long long)kb * taps + tap) * ksteps + s;
-    long long base = step * (4LL * NT * 8);      // halfs per step: hi 2*NT*8 + lo 2*NT*8
+    long long base = step * (2LL * parts * NT * 8);      // halfs per step: hi 2*NT*8 [+ lo 2*NT*8]
     long long o = (long long)(j * NT + n) * 8 + e;
     out[base + o] = h;
-    out[base + 2LL * NT * 8 + o] = l;
+    if (parts == 2) out[base + 2LL * NT * 8 + o] = l;
   }
 }
 
@@ -546,9 +559,10 @@ constexpr size_t SMEM_LIMIT = 227 * 1024;
 size_t round1024(size_t x) { return (x + 1023) & ~(size_t)1023; }
 
 // shared-memory plan of one conv with MT-position tiles and SA slab stages (two raw stages where they fit); false
-// when it does not fit.  Layout: slab stages, weight stages, raw stages (1024-byte aligned for the swizzled TMA
-// boxes), position table, statistics, barriers.
-bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, int MT, Plan& p) {
+// when it does not fit.  vbytes = staged bytes per operand value: 4 (fp16 hi + lo) or 2 (half mode, hi only).
+// Layout: slab stages, weight stages, raw stages (1024-byte aligned for the swizzled TMA boxes), position table,
+// statistics, barriers.
+bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, int MT, int vbytes, Plan& p) {
   const int Wp = ks == 3 ? W + 1 : W;
   const int Pimg = ks == 3 ? (H + 1) * (W + 1) : H * W;
   const int halo0 = ks == 3 ? Wp + 1 : 0;
@@ -560,8 +574,8 @@ bool make_plan(int H, int W, int ks, int KB, int NT, bool stats, int SA, int MT,
   p.tab_nb = std::min(p.HP / Pimg + 2, TAB_NB);
   p.tab_off = p.nbox * p.boxn * KB * 4;
   p.raw_stage = (int)round1024((size_t)p.tab_off + (size_t)p.tab_nb * KB * 16);
-  const size_t a_stage = (size_t)2 * (KB / 8) * p.HP * 16;
-  const size_t b_stage = (size_t)(KB / 16) * 64 * NT;
+  const size_t a_stage = (size_t)(KB / 8) * p.HP * 8 * vbytes;
+  const size_t b_stage = (size_t)(KB / 16) * 16 * vbytes * NT;
   const size_t stat_bytes = stats ? (size_t)p.NJ * 2 * NT * 8 : 0;
   const size_t pinfo_bytes = (size_t)PPT * NPROD * 4;
   size_t bar_bytes = 0, fixed = 0;
@@ -614,20 +628,26 @@ int encode_map(CUtensorMap* m, const float* base, int rank, const cuuint64_t* di
   return 0;
 }
 
-template <int NT, int NWG>
+template <int NT, int NWG, bool HALF>
 int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, cudaStream_t s) {
-  cudaError_t e = cudaFuncSetAttribute(k_conv_umma<NT, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e =
+      cudaFuncSetAttribute(k_conv_umma<NT, NWG, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   MCVD_CHECK(e == cudaSuccess, "CONV_UMMA: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-  k_conv_umma<NT, NWG><<<grid, 128 * (NWG + 1), smem, s>>>(a, m);
+  k_conv_umma<NT, NWG, HALF><<<grid, 128 * (NWG + 1), smem, s>>>(a, m);
   MCVD_CUDA_LAUNCH_CHECK("conv_umma");
   return 0;
 }
 
-template <int NT>
+template <int NT, bool HALF>
 int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, int nwg, cudaStream_t s) {
   if constexpr (NT <= NT_MAX3)
-    if (nwg == 3) return launch_nt<NT, 3>(a, m, smem, grid, s);
-  return launch_nt<NT, 2>(a, m, smem, grid, s);
+    if (nwg == 3) return launch_nt<NT, 3, HALF>(a, m, smem, grid, s);
+  return launch_nt<NT, 2, HALF>(a, m, smem, grid, s);
+}
+
+template <int NT>
+int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, int nwg, bool half, cudaStream_t s) {
+  return half ? launch_nt<NT, true>(a, m, smem, grid, nwg, s) : launch_nt<NT, false>(a, m, smem, grid, nwg, s);
 }
 
 // common launcher: planar = the CONV_UMMA2 variant (planar norm table, K-block fixed by the caller when i2 != 0,
@@ -651,6 +671,10 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
              op.i2, a.KB);
   MCVD_CHECK(NT >= 16 && NT <= 256 && NT % 16 == 0 && op.Cout % NT == 0, "%s: n tile %d invalid for Cout %d", name, NT,
              op.Cout);
+  const bool half = (op.flags & MCVD_F_HALF) != 0;
+  MCVD_CHECK(!half || op.i3 == 0 || op.i3 == 3, "%s: operand split %d with MCVD_F_HALF (one product; 0 or 3)", name,
+             op.i3);
+  const int vbytes = half ? 2 : 4;
   if (a.ks == 3) { a.Wp = op.W + 1; a.Pimg = (op.H + 1) * (op.W + 1); }
   else { a.Wp = op.W; a.Pimg = op.H * op.W; }
   MCVD_CHECK((long long)op.B * a.Pimg < (1LL << 31), "%s: too many pixels", name);
@@ -676,7 +700,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   MCVD_CHECK(mode >= 0 && mode <= 2, "%s: work organisation %d", name, mode);
   Plan p;
   const bool can_stay = a.ks == 1 && a.nKB == a.nKB0 && a.tiles_n > 1 && a.nKB <= MAX_RESIDENT &&
-                        make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, STAT_MT, p);
+                        make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, STAT_MT, vbytes, p);
   const bool stay = can_stay && (mode == 2 || (mode == 0 && 2 * tiles128 >= sms));
   // Slab stages of a streaming conv (CONV_UMMA i5, diagnostics): 0 = the launcher's choice, 2 or 3 forces them.
   const int sa_req = planar ? 0 : op.i5;
@@ -697,7 +721,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   const int mt_req = planar ? 0 : op.i4;
   MCVD_CHECK(mt_req == 0 || mt_req == 128 || mt_req == 192, "%s: tile height %d", name, mt_req);
   const bool can3 = !planar && NT <= NT_MAX3 && !stay && !a.stats &&
-                    make_plan(op.H, op.W, a.ks, a.KB, NT, false, a.SA, 192, p) &&
+                    make_plan(op.H, op.W, a.ks, a.KB, NT, false, a.SA, 192, vbytes, p) &&
                     (!a.tab || p.HP / a.Pimg + 2 <= TAB_NB);
   MCVD_CHECK(mt_req != 192 || can3, "%s: 192-position tiles need streaming, NT <= %d, no statistics and %dx%d to fit",
              name, NT_MAX3, op.H, op.W);
@@ -708,7 +732,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   const int MT = mt_req ? mt_req : (can3 && p.NB >= 3 && last_positions(192) <= last_positions(128) ? 192 : 128);
   long long tiles_m = (a.Qtot + MT - 1) / MT;
   if (planar) tiles_m = (tiles_m + 1) & ~1LL;          // the statistics array is sized in tile pairs: write all of it
-  MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, MT, p),
+  MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, MT, vbytes, p),
              "%s: tile does not fit shared memory (W=%d)", name, op.W);
   a.HP = p.HP; a.NB = p.NB; a.NJ = p.NJ;
   a.boxn = p.boxn; a.nbox = p.nbox; a.raw_off = p.raw_off; a.raw_stage = p.raw_stage; a.tab_off = p.tab_off;
@@ -756,7 +780,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   a.ntiles = (int)(tiles_m * (a.tiles_n / a.NPI));
   const int grid = a.ntiles < sms ? a.ntiles : sms;
   switch (NT) {
-#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, maps, p.smem, grid, MT / 64, s);
+#define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, maps, p.smem, grid, MT / 64, half, s);
     MCVD_NT_CASE(16) MCVD_NT_CASE(32) MCVD_NT_CASE(48) MCVD_NT_CASE(64) MCVD_NT_CASE(80) MCVD_NT_CASE(96)
     MCVD_NT_CASE(112) MCVD_NT_CASE(128) MCVD_NT_CASE(144) MCVD_NT_CASE(160) MCVD_NT_CASE(176) MCVD_NT_CASE(192)
     MCVD_NT_CASE(208) MCVD_NT_CASE(224) MCVD_NT_CASE(240) MCVD_NT_CASE(256)
@@ -767,12 +791,16 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
 }
 
 long long pack(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB, void* out, int scale_log2,
-               int stage_off, int per_unit, void* stream) {
+               int stage_off, int per_unit, int parts, void* stream) {
   if ((KB != 16 && KB != 32) || Cin % KB || n_tile < 16 || n_tile % 16 || Cout % n_tile) {
     set_error("umma_pack_weights: Cin %d / Cout %d / n_tile %d / KB %d unsupported", Cin, Cout, n_tile, KB);
     return -1;
   }
-  const long long bytes = (long long)taps * Cin * Cout * 4;      // hi + lo fp16
+  if (parts != 1 && parts != 2) {
+    set_error("umma_pack_weights: parts %d (1 = hi, 2 = hi + lo)", parts);
+    return -1;
+  }
+  const long long bytes = (long long)taps * Cin * Cout * 2 * parts;      // fp16 hi [+ lo]
   if (!out) return bytes;
   if (!w_taps) {
     set_error("umma_pack_weights: null input");
@@ -783,7 +811,7 @@ long long pack(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int
   long long blocks = (total + 255) / 256;
   if (blocks > 132LL * 16) blocks = 132LL * 16;
   k_pack_weights<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(w_taps, (__half*)out, taps, Cin, Cout, n_tile, KB,
-                                                                      scale, stage_off, per_unit);
+                                                                      scale, stage_off, per_unit, parts);
   if (cudaGetLastError() != cudaSuccess) {
     set_error("umma_pack_weights: launch failed");
     return -2;
@@ -802,14 +830,20 @@ extern "C" int mcvd_umma_kblock(int C0, int C1) { return mcvd::pick_kb(C0, C1); 
 
 extern "C" long long mcvd_umma_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB,
                                             void* out, int scale_log2, void* stream) {
-  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, 0, KB ? (Cin / KB) * taps : 0, stream);
+  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, 0, KB ? (Cin / KB) * taps : 0, 2, stream);
+}
+
+extern "C" long long mcvd_umma_pack_weights_ex(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB,
+                                               void* out, int scale_log2, int stage_off, int per_unit, int parts,
+                                               void* stream) {
+  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, stage_off, per_unit, parts, stream);
 }
 
 extern "C" int mcvd_umma2_plan(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats) {
   const int kb = mcvd::conv_kb(C0, C1, C2, C3);
   mcvd::Plan p;
   if (!kb || n_tile < 16 || n_tile > 256 || n_tile % 16) return 0;
-  return mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, mcvd::STAT_MT, p) ? kb : 0;
+  return mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, mcvd::STAT_MT, 4, p) ? kb : 0;
 }
 
 // shared-memory plan of a conv (diagnostics / tests): out[0..9] = KB, HP, image stages, raw-input stages, weight
@@ -820,7 +854,7 @@ extern "C" int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2
   const int kb = mcvd_umma2_plan(H, W, ks, C0, C1, C2, C3, n_tile, stats);
   if (!kb || !out) return -1;
   mcvd::Plan p;
-  mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, mcvd::STAT_MT, p);
+  mcvd::make_plan(H, W, ks, kb, n_tile, stats != 0, 2, mcvd::STAT_MT, 4, p);
   out[0] = kb; out[1] = p.HP; out[2] = 2; out[3] = p.RA; out[4] = p.NB; out[5] = p.NJ; out[6] = 0;
   out[7] = (int)p.smem; out[8] = 1; out[9] = 1;
   return 0;
@@ -835,5 +869,5 @@ extern "C" long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cou
 
 extern "C" long long mcvd_umma2_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int KB,
                                              void* out, int scale_log2, int stage_off, int per_unit, void* stream) {
-  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, stage_off, per_unit, stream);
+  return mcvd::pack(w_taps, taps, Cin, Cout, n_tile, KB, out, scale_log2, stage_off, per_unit, 2, stream);
 }

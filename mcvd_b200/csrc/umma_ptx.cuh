@@ -143,5 +143,13 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - hf.y), "f"(a - hf.x));
 }
 
+
+// half mode: the hi parts of split2 only (same saturating rounding)
+__device__ __forceinline__ uint32_t cvt_hi2(float a, float b) {
+  uint32_t hi;
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
+  return hi;
+}
+
 }  // namespace ptx
 }  // namespace mcvd

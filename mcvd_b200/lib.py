@@ -60,11 +60,12 @@ F_GAMMA = 1 << 8
 F_POOL = 1 << 9
 F_L1 = 1 << 10
 F_AVG = 1 << 11
+F_HALF = 1 << 12
 
 ABI_VERSION = 5
 
 EXPORTS = ["mcvd_abi_version", "mcvd_sizeof_op", "mcvd_last_error", "mcvd_device_arch", "mcvd_run_program",
-           "mcvd_validate_program", "mcvd_count_launches", "mcvd_umma_pack_weights", "mcvd_umma_kblock",
+           "mcvd_validate_program", "mcvd_count_launches", "mcvd_umma_pack_weights", "mcvd_umma_pack_weights_ex", "mcvd_umma_kblock",
            "mcvd_attention_scratch_bytes", "mcvd_umma2_plan", "mcvd_umma2_plan_info", "mcvd_umma2_stats_bytes", "mcvd_umma2_pack_weights",
            "mcvd_tf32_packed_bytes", "mcvd_tf32_pack_weights"]
 
@@ -131,6 +132,9 @@ def load():
         lib.mcvd_umma_pack_weights.restype = C.c_longlong
         lib.mcvd_umma_pack_weights.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                                C.c_int, C.c_void_p]
+        lib.mcvd_umma_pack_weights_ex.restype = C.c_longlong
+        lib.mcvd_umma_pack_weights_ex.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                                  C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
         lib.mcvd_umma_kblock.restype = C.c_int
         lib.mcvd_umma_kblock.argtypes = [C.c_int, C.c_int]
         lib.mcvd_attention_scratch_bytes.restype = C.c_longlong

@@ -125,6 +125,7 @@ class UNetMore_DDPM(nn.Module):
         if why is not None:
             raise NotImplementedError(f"mcvd_b200 does not accelerate this configuration: {why}")
         self.config = config
+        self.conv_precision = arch.conv_precision(config)      # not part of the state_dict
         self.version = getattr(config.model, "version", "DDPM").upper()
         self.spec = arch.build_spec(config)
         self.unet = _UNet(config, self.spec)

@@ -142,6 +142,9 @@ class Engine:
         self.packs_computed = 0
         self.packs_loaded = 0
         self.programs: Dict[int, Program] = {}
+        # model.conv_precision, read once: "fp16" gives the convs that lower the reference's nn.Conv2d layers (first
+        # and final conv, Conv_0/1/2, SPADE) MCVD_F_HALF and hi-only weight images; NIN projections keep fp32 parity
+        self.conv_precision = getattr(module, "conv_precision", "fp32")
         self.launches_last_forward = 0
         self.launches_last_dsm = 0
 
@@ -175,7 +178,10 @@ class Engine:
         import hashlib
         ids, fp = self.packed_version
         h = hashlib.sha256()
-        h.update(repr((lib.ABI_VERSION, self.conv_mode, self.split_mode, [sh for _, sh in ids])).encode())
+        mode = (lib.ABI_VERSION, self.conv_mode, self.split_mode, [sh for _, sh in ids])
+        if self.conv_precision != "fp32":                 # fp32 cache files keep their names
+            mode = mode + (self.conv_precision,)
+        h.update(repr(mode).encode())
         h.update(fp.detach().cpu().numpy().tobytes())
         return os.path.join(self.cache_dir, f"mcvd_b200_packed_{h.hexdigest()[:32]}.pt")
 
@@ -250,21 +256,26 @@ class Engine:
     def _devctx(self):
         return torch.cuda.device(self.device) if self.device.type == "cuda" else contextlib.nullcontext()
 
-    def _pack_umma(self, taps: torch.Tensor, nt: int, kb: int):
+    def _pack_image(self, t: torch.Tensor, nt: int, kb: int, k: int, half: bool) -> torch.Tensor:
+        """one stand-alone CONV_UMMA weight image of fp32 taps [T][I][O]: fp16 hi/lo, or hi only with ``half``"""
+        T, I, O = t.shape
+        parts = 1 if half else 2
+        out = torch.empty(T * I * O * 2 * parts, device=t.device, dtype=torch.uint8)
+        with self._devctx():
+            rc = self.lib.mcvd_umma_pack_weights_ex(t.data_ptr(), T, I, O, nt, kb, out.data_ptr(), k, 0, (I // kb) * T,
+                                                    parts, self._stream())
+        if rc < 0:
+            raise RuntimeError(f"mcvd_b200 umma_pack_weights failed: {lib.last_error()}")
+        return out
+
+    def _pack_umma(self, taps: torch.Tensor, nt: int, kb: int, half: bool = False):
         if self.backend is not None:
             return self.backend.pack_umma(taps, nt, kb)
         self.packs_computed += 1
-        T, I, O = taps.shape
         k = umma_scale_log2(float(taps.abs().max().item()))
-        out = torch.empty(T * I * O * 4, device=taps.device, dtype=torch.uint8)
-        stream = self._stream()
-        with self._devctx():
-            rc = self.lib.mcvd_umma_pack_weights(taps.data_ptr(), T, I, O, nt, kb, out.data_ptr(), k, stream)
-        if rc < 0:
-            raise RuntimeError(f"mcvd_b200 umma_pack_weights failed: {lib.last_error()}")
-        return out, float(2.0 ** (-k))
+        return self._pack_image(taps, nt, kb, k, half), float(2.0 ** (-k))
 
-    def _pack_umma_fused(self, taps: torch.Tensor, taps_sc: torch.Tensor, nt: int, kb: int):
+    def _pack_umma_fused(self, taps: torch.Tensor, taps_sc: torch.Tensor, nt: int, kb: int, half: bool = False):
         """main conv + 1x1 shortcut as one weight stream: per n-tile [main stages | shortcut stages]."""
         if self.backend is not None:
             both = torch.cat([taps.reshape(-1), taps_sc.reshape(-1)]).contiguous()
@@ -273,18 +284,10 @@ class Engine:
         self.packs_computed += 1
         k = umma_scale_log2(float(max(taps.abs().max().item(), taps_sc.abs().max().item())))
         n_nt = taps.shape[2] // nt
-        parts = []
-        for t in (taps, taps_sc):
-            T, I, O = t.shape
-            out = torch.empty(T * I * O * 4, device=t.device, dtype=torch.uint8)
-            with self._devctx():
-                rc = self.lib.mcvd_umma_pack_weights(t.data_ptr(), T, I, O, nt, kb, out.data_ptr(), k, self._stream())
-            if rc < 0:
-                raise RuntimeError(f"mcvd_b200 umma_pack_weights failed: {lib.last_error()}")
-            parts.append(out.view(n_nt, -1))
+        parts = [self._pack_image(t, nt, kb, k, half).view(n_nt, -1) for t in (taps, taps_sc)]
         return torch.cat(parts, dim=1).contiguous().view(-1), float(2.0 ** (-k))
 
-    def _pack_umma2(self, taps: torch.Tensor, taps_sc: Optional[torch.Tensor], nt: int, kb: int):
+    def _pack_umma2(self, taps: torch.Tensor, taps_sc: Optional[torch.Tensor], nt: int, kb: int, half: bool = False):
         """Weight images of the planar-table conv variant: main conv stages, then the fused 1x1 shortcut's, per n tile."""
         if self.backend is not None:
             flat = taps.reshape(-1) if taps_sc is None else torch.cat([taps.reshape(-1), taps_sc.reshape(-1)])
@@ -298,13 +301,14 @@ class Engine:
         T, I, O = taps.shape
         isc = 0 if taps_sc is None else taps_sc.shape[1]
         per_unit = (I // kb) * T + isc // kb
-        out = torch.empty((T * I + isc) * O * 4, device=taps.device, dtype=torch.uint8)
+        parts = 1 if half else 2
+        out = torch.empty((T * I + isc) * O * 2 * parts, device=taps.device, dtype=torch.uint8)
         with self._devctx():
-            rc = self.lib.mcvd_umma2_pack_weights(taps.data_ptr(), T, I, O, nt, kb, out.data_ptr(), k, 0, per_unit,
-                                                  self._stream())
+            rc = self.lib.mcvd_umma_pack_weights_ex(taps.data_ptr(), T, I, O, nt, kb, out.data_ptr(), k, 0, per_unit,
+                                                    parts, self._stream())
             if rc >= 0 and taps_sc is not None:
-                rc = self.lib.mcvd_umma2_pack_weights(taps_sc.data_ptr(), 1, isc, O, nt, kb, out.data_ptr(), k,
-                                                      (I // kb) * T, per_unit, self._stream())
+                rc = self.lib.mcvd_umma_pack_weights_ex(taps_sc.data_ptr(), 1, isc, O, nt, kb, out.data_ptr(), k,
+                                                        (I // kb) * T, per_unit, parts, self._stream())
         if rc < 0:
             raise RuntimeError(f"mcvd_b200 umma2_pack_weights failed: {lib.last_error()}")
         return out, float(2.0 ** (-k))
@@ -350,6 +354,7 @@ class Engine:
         dev = self.device
         P = Program()
         P.B = B
+        P.conv_precision = self.conv_precision
         S = ns.image_size
 
         def f32(*shape):
@@ -383,7 +388,11 @@ class Engine:
                  scale=1.0, tab=None, act_in=False, act_out=False, nin=False, wcat=None, bcat=None, shortcut=None,
                  stats=False):
             """dst = scale * (conv(act(norm(src))) + bias + residual [+ conv1x1(shortcut src)]).
-            stats: the output feeds a GroupNorm -- let the conv epilogue emit its partial sums."""
+            stats: the output feeds a GroupNorm -- let the conv epilogue emit its partial sums.  nin: the op lowers
+            an NIN projection (a matmul in the reference), which never takes the half mode."""
+            half = self.conv_precision == "fp16" and not nin
+            fl_half = lib.F_HALF if half else 0
+            ptag = ("fp16",) if half else ()                 # packed-image key: fp32 keys are unchanged
             if wcat is not None:
                 taps, bias = wcat, bcat
             elif nin:
@@ -409,11 +418,11 @@ class Engine:
                     if shortcut is not None:
                         sc_taps = self._conv_taps(sd(sc_w))
                         bias = keep((bias + sd(sc_b).float()).contiguous())
-                    pk = (key, "umma2", nt, kb, shortcut is not None)
+                    pk = (key, "umma2", nt, kb, shortcut is not None) + ptag
                     if pk not in self.packed:
-                        self.packed[pk] = self._pack_umma2(taps, sc_taps, nt, kb)
+                        self.packed[pk] = self._pack_umma2(taps, sc_taps, nt, kb, half)
                     wp, wscale = self.packed[pk]
-                    fl = (lib.F_ACT_IN if act_in else 0) | (lib.F_ACT_OUT if act_out else 0)
+                    fl = (lib.F_ACT_IN if act_in else 0) | (lib.F_ACT_OUT if act_out else 0) | fl_half
                     kw2 = {}
                     if shortcut is not None:
                         kw2 = dict(src2=sc_src.t0, src3=sc_src.t1, C2=c2, C3=c3)
@@ -423,7 +432,7 @@ class Engine:
                                               dtype=torch.int64))
                         stats_of[dst.data_ptr()] = (st, ks)
                     emit(ops, lib.OP_CONV_UMMA2, H=H, W=H, C0=src.c0, C1=src.c1, Cout=cout, i0=ks, i1=nt, i2=kb,
-                         i3=self.split_mode, f0=scale, f1=wscale, src0=src.t0, src1=src.t1, w=wp, bias=bias,
+                         i3=3 if half else self.split_mode, f0=scale, f1=wscale, src0=src.t0, src1=src.t1, w=wp, bias=bias,
                          aux0=residual, aux1=None if tab is None else tab3_of[tab.data_ptr()], dst=dst, dst2=st,
                          flags=fl, **kw2)
                     P.n_umma += 1
@@ -443,15 +452,15 @@ class Engine:
                     assert residual is None
                     residual = conv(ops, key + ".sc", sc_src, H, cout, 1, sc_w, sc_b)
             if kb and nt and (tab is None or H >= 8):      # fused-norm slab stages <= 8 images' table rows
-                pk = (key, "umma", nt, kb, sc is not None)
+                pk = (key, "umma", nt, kb, sc is not None) + ptag
                 if pk not in self.packed:
                     if sc is None:
-                        self.packed[pk] = self._pack_umma(taps, nt, kb)
+                        self.packed[pk] = self._pack_umma(taps, nt, kb, half)
                     else:                                  # both segments share one power-of-two scale
-                        self.packed[pk] = self._pack_umma_fused(taps, sc[1], nt, kb)
+                        self.packed[pk] = self._pack_umma_fused(taps, sc[1], nt, kb, half)
                 wp, wscale = self.packed[pk]
                 nacc = 0                       # work organisation: the launcher's choice (input-stationary 1x1 / streaming)
-                fl = (lib.F_ACT_IN if act_in else 0) | (lib.F_ACT_OUT if act_out else 0)
+                fl = (lib.F_ACT_IN if act_in else 0) | (lib.F_ACT_OUT if act_out else 0) | fl_half
                 kw2 = {}
                 if sc is not None:
                     kw2 = dict(src2=sc[0].t0, src3=sc[0].t1, C2=sc[0].c0, C3=sc[0].c1)
@@ -461,7 +470,8 @@ class Engine:
                     st = keep(torch.zeros(lib.umma2_stats_bytes(B, H, H, ks, cout) // 8, device=dev, dtype=torch.int64))
                     stats_of[dst.data_ptr()] = (st, ks)
                 emit(ops, lib.OP_CONV_UMMA, H=H, W=H, C0=src.c0, C1=src.c1, Cout=cout, i0=ks, i1=nt, i2=nacc,
-                     i3=self.split_mode, f0=scale, f1=wscale, src0=src.t0, src1=src.t1, w=wp, bias=bias, aux0=residual, aux1=tab,
+                     i3=3 if half else self.split_mode, f0=scale, f1=wscale, src0=src.t0, src1=src.t1, w=wp, bias=bias,
+                     aux0=residual, aux1=tab,
                      dst=dst, dst2=st, flags=fl, **kw2)
                 P.n_umma += 1
                 return dst
@@ -633,7 +643,8 @@ class Engine:
                              affine=(sd(pre + "GroupNorm_0.weight"), sd(pre + "GroupNorm_0.bias")))
             wq = torch.cat([sd(pre + f"NIN_{i}.W").float() for i in range(3)], dim=1).unsqueeze(0).contiguous()
             bq = torch.cat([sd(pre + f"NIN_{i}.b").float() for i in range(3)], dim=0).contiguous()
-            qkv = conv(step, pre + "qkv", Src(x, C), H, 3 * C, 1, None, None, tab=tab, act_in=False, wcat=wq, bcat=bq)
+            qkv = conv(step, pre + "qkv", Src(x, C), H, 3 * C, 1, None, None, tab=tab, act_in=False, nin=True, wcat=wq,
+                       bcat=bq)
             att = f32(B, H, H, C)
             d = C // ms.heads
             T = H * H

@@ -1,12 +1,13 @@
 """Time every tensor-core conv launch of one forward of a workload (default cfg2, B = 64) with CUDA events, grouped by
 (ks, H, Cin | Csc, Cout, NT): microseconds per forward, algorithmic and executed TFLOP/s, and share of the forward.
 Algorithmic work counts 2 * pixels * Cout * (Cin * ks^2 + Csc); executed work counts every padded-flat position row
-(padding positions included) rounded up to whole 128-position tiles, and the three fp16 products of the hi/lo split.
+(padding positions included) rounded up to whole 128-position tiles, and the three fp16 products of the hi/lo split
+(one product for the half-mode convs of --precision fp16).
 Convs the launcher runs in 192-position tiles execute up to 191 rather than 127 rows past the last position, which
 this count leaves out (under 0.4 % of the rows at 16x16 and above for the default batch).  The GPU name and power
 limit are read (not set) in the same run.
 
-    python tools/time_conv.py [--workload cfg2] [--batch 64] [--reps 20]
+    python tools/time_conv.py [--workload cfg2] [--batch 64] [--reps 20] [--precision fp32|fp16]
 """
 import argparse
 import collections
@@ -40,13 +41,15 @@ def main():
     ap.add_argument("--workload", default="cfg2")
     ap.add_argument("--batch", type=int, default=0)
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--precision", default="fp32", choices=["fp32", "fp16"], help="model.conv_precision")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "time_conv.py measures on a CUDA device"
     q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True).stdout.strip()
     cfg = configs.workload(args.workload)
     B = args.batch or cfg.bench_batch
-    _, net, _ = make_module(args.workload, "cuda:0")
+    cfg.model.conv_precision = args.precision
+    _, net, _ = make_module(cfg, "cuda:0")
     P = net.engine().program(B)
     ops = list(P.step_ops)
     fwd = time_ops(ops, args.reps)
@@ -59,12 +62,12 @@ def main():
         pimg = (op.H + 1) * (op.W + 1) if ks == 3 else op.H * op.W
         rows = -(-op.B * pimg // 128) * 128
         alg = 2.0 * op.B * op.H * op.W * op.Cout * (cin * ks * ks + csc)
-        exe = 3 * 2.0 * rows * op.Cout * (cin * ks * ks + csc)
+        exe = (1 if op.flags & lib.F_HALF else 3) * 2.0 * rows * op.Cout * (cin * ks * ks + csc)
         key = (ks, op.H, cin, csc, op.Cout, op.i1)
         g = groups.setdefault(key, [0, 0.0, 0.0, 0.0])
         g[0] += 1; g[1] += us; g[2] += alg; g[3] += exe
     print(f"GPU: {q}")
-    print(f"{args.workload} B={B}: forward {fwd:.0f} us ({len(ops)} ops)")
+    print(f"{args.workload} B={B} conv_precision={args.precision}: forward {fwd:.0f} us ({len(ops)} ops)")
     print(f"{'ks':>2} {'H':>4} {'Cin|Csc':>9} {'Cout':>5} {'NT':>4} {'n':>3} {'us':>9} {'alg_TF/s':>9} {'exe_TF/s':>9} {'share':>6}")
     tot = 0.0
     for (ks, H, cin, csc, cout, nt), (n, us, alg, exe) in groups.items():
