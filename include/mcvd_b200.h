@@ -358,6 +358,11 @@ int mcvd_umma2_plan(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_
  * slab rows, image stages, raw-ring stages, weight stages, image slots per tile, 0, dynamic shared
  * memory bytes.  Returns 0, or -1 when the conv cannot run on this kernel. */
 int mcvd_umma2_plan_info(int H, int W, int ks, int C0, int C1, int C2, int C3, int n_tile, int stats, int* out);
+/* The launch plan MCVD_OP_CONV_UMMA / MCVD_OP_CONV_UMMA2 op `op` gets on a GPU of `sms` SMs (diagnostics / tests; host
+ * arithmetic only, computed by the launcher's own planning code): out[0..8] = K-block, tile height (positions),
+ * slab stages, weight stages, raw-input stages, n tiles per work item (> 1: input-stationary), work items, grid,
+ * dynamic shared memory bytes.  Returns 0, or -1 with the launcher's error text (mcvd_last_error). */
+int mcvd_conv_umma_launch_info(const McvdOp* op, int sms, int* out);
 /* Bytes of the dst2 statistics array of a MCVD_OP_CONV_UMMA2 op. */
 long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cout);
 /* Weight packing for MCVD_OP_CONV_UMMA2 (the MCVD_OP_CONV_UMMA layout).  w_taps = fp32 [taps][Cin][Cout]; every

@@ -650,13 +650,13 @@ int launch_nt(const ConvArgs& a, const ConvMaps& m, size_t smem, int grid, int n
   return half ? launch_nt<NT, true>(a, m, smem, grid, nwg, s) : launch_nt<NT, false>(a, m, smem, grid, nwg, s);
 }
 
-// common launcher: planar = the CONV_UMMA2 variant (planar norm table, K-block fixed by the caller when i2 != 0,
-// statistics tiles padded to pairs)
-int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
+// Launch plan of one conv on `sms` SMs: the kernel arguments, the shared-memory plan, the tile height and the grid.
+// Host arithmetic only; launch_conv runs exactly this plan.  planar = the CONV_UMMA2 variant (planar norm table,
+// K-block fixed by the caller when i2 != 0, statistics tiles padded to pairs).
+int plan_conv(const McvdOp& op, int sms, bool planar, ConvArgs& a, Plan& p, int& MT, int& grid) {
   const char* name = planar ? "CONV_UMMA2" : "CONV_UMMA";
   MCVD_CHECK(op.src0 && op.w && op.dst && (op.C1 == 0 || op.src1), "%s: null pointer", name);
   MCVD_CHECK(op.i0 == 1 || op.i0 == 3, "%s: kernel size %d unsupported", name, op.i0);
-  ConvArgs a;
   a.s0 = (const float*)op.src0; a.s1 = (const float*)op.src1; a.wpk = (const __half*)op.w;
   a.s2 = (const float*)op.src2; a.s3 = (const float*)op.src3; a.C2 = op.src2 ? op.C2 : 0; a.C3 = op.src3 ? op.C3 : 0;
   a.bias = (const float*)op.bias; a.res = (const float*)op.aux0; a.tab = (const float*)op.aux1;
@@ -685,9 +685,6 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   a.nKB = a.nKB0 + (a.C2 + a.C3) / a.KB;
   a.tiles_n = op.Cout / NT;
   const long long tiles128 = (a.Qtot + STAT_MT - 1) / STAT_MT;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   // Work organisation (CONV_UMMA i2): 1 = streaming, one (m tile, n tile) per work item through two slab stages;
   // 2 = input-stationary, one m tile per work item with its whole input resident (one slab stage per K-block) while
   // the weights of every n tile stream past it, so the input is read and transformed once instead of once per n
@@ -698,7 +695,6 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
   // tools/time_conv1x1.py repeats the measurement.
   const int mode = planar ? 0 : op.i2;
   MCVD_CHECK(mode >= 0 && mode <= 2, "%s: work organisation %d", name, mode);
-  Plan p;
   const bool can_stay = a.ks == 1 && a.nKB == a.nKB0 && a.tiles_n > 1 && a.nKB <= MAX_RESIDENT &&
                         make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.nKB, STAT_MT, vbytes, p);
   const bool stay = can_stay && (mode == 2 || (mode == 0 && 2 * tiles128 >= sms));
@@ -729,7 +725,7 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
     const long long items = (a.Qtot + mt - 1) / mt * a.tiles_n;
     return (items + sms - 1) / sms * mt;
   };
-  const int MT = mt_req ? mt_req : (can3 && p.NB >= 3 && last_positions(192) <= last_positions(128) ? 192 : 128);
+  MT = mt_req ? mt_req : (can3 && p.NB >= 3 && last_positions(192) <= last_positions(128) ? 192 : 128);
   long long tiles_m = (a.Qtot + MT - 1) / MT;
   if (planar) tiles_m = (tiles_m + 1) & ~1LL;          // the statistics array is sized in tile pairs: write all of it
   MCVD_CHECK(make_plan(op.H, op.W, a.ks, a.KB, NT, a.stats != nullptr, a.SA, MT, vbytes, p),
@@ -746,6 +742,23 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
     MCVD_CHECK(nb <= TAB_NB || !a.tab, "%s: %dx%d images are too small for the fused-norm path", name, op.H, op.W);
     a.tab_nb = (nb <= TAB_NB) ? nb : 0;
   }
+  MCVD_CHECK(tiles_m * a.tiles_n < (1LL << 31), "%s: too many tiles", name);
+  a.ntiles = (int)(tiles_m * (a.tiles_n / a.NPI));
+  grid = a.ntiles < sms ? a.ntiles : sms;
+  return 0;
+}
+
+int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
+  const char* name = planar ? "CONV_UMMA2" : "CONV_UMMA";
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  ConvArgs a;
+  Plan p;
+  int MT = 0, grid = 0;
+  if (plan_conv(op, sms, planar, a, p, MT, grid)) return -1;
+  const int NT = op.i1;
+  const bool half = (op.flags & MCVD_F_HALF) != 0;
   // TMA maps: sources as {C, B*H*W} rows of KB channels, swizzled; the norm table as {4*Cin, B} or {Cin, 3, B}
   ConvMaps maps;
   memset(&maps, 0, sizeof(maps));
@@ -776,9 +789,6 @@ int launch_conv(const McvdOp& op, cudaStream_t s, bool planar) {
       }
     }
   }
-  MCVD_CHECK(tiles_m * a.tiles_n < (1LL << 31), "%s: too many tiles", name);
-  a.ntiles = (int)(tiles_m * (a.tiles_n / a.NPI));
-  const int grid = a.ntiles < sms ? a.ntiles : sms;
   switch (NT) {
 #define MCVD_NT_CASE(n) case n: return launch_nt<n>(a, maps, p.smem, grid, MT / 64, half, s);
     MCVD_NT_CASE(16) MCVD_NT_CASE(32) MCVD_NT_CASE(48) MCVD_NT_CASE(64) MCVD_NT_CASE(80) MCVD_NT_CASE(96)
@@ -825,6 +835,20 @@ int launch_conv_umma(const McvdOp& op, cudaStream_t s) { return launch_conv(op, 
 int launch_conv_umma2(const McvdOp& op, cudaStream_t s) { return launch_conv(op, s, true); }
 
 }  // namespace mcvd
+
+extern "C" int mcvd_conv_umma_launch_info(const McvdOp* op, int sms, int* out) {
+  if (!op || !out || sms < 1 || (op->kind != MCVD_OP_CONV_UMMA && op->kind != MCVD_OP_CONV_UMMA2)) {
+    mcvd::set_error("conv_umma_launch_info: needs a CONV_UMMA or CONV_UMMA2 op, an output array and sms >= 1");
+    return -1;
+  }
+  mcvd::ConvArgs a;
+  mcvd::Plan p;
+  int MT = 0, grid = 0;
+  if (mcvd::plan_conv(*op, sms, op->kind == MCVD_OP_CONV_UMMA2, a, p, MT, grid)) return -1;
+  out[0] = a.KB; out[1] = MT; out[2] = a.SA; out[3] = a.NB; out[4] = a.RA; out[5] = a.NPI; out[6] = a.ntiles;
+  out[7] = grid; out[8] = (int)p.smem;
+  return 0;
+}
 
 extern "C" int mcvd_umma_kblock(int C0, int C1) { return mcvd::pick_kb(C0, C1); }
 

@@ -66,7 +66,7 @@ ABI_VERSION = 5
 
 EXPORTS = ["mcvd_abi_version", "mcvd_sizeof_op", "mcvd_last_error", "mcvd_device_arch", "mcvd_run_program",
            "mcvd_validate_program", "mcvd_count_launches", "mcvd_umma_pack_weights", "mcvd_umma_pack_weights_ex", "mcvd_umma_kblock",
-           "mcvd_attention_scratch_bytes", "mcvd_umma2_plan", "mcvd_umma2_plan_info", "mcvd_umma2_stats_bytes", "mcvd_umma2_pack_weights",
+           "mcvd_attention_scratch_bytes", "mcvd_umma2_plan", "mcvd_umma2_plan_info", "mcvd_conv_umma_launch_info", "mcvd_umma2_stats_bytes", "mcvd_umma2_pack_weights",
            "mcvd_tf32_packed_bytes", "mcvd_tf32_pack_weights"]
 
 
@@ -143,6 +143,8 @@ def load():
         lib.mcvd_umma2_plan.argtypes = [C.c_int] * 9
         lib.mcvd_umma2_plan_info.restype = C.c_int
         lib.mcvd_umma2_plan_info.argtypes = [C.c_int] * 9 + [C.POINTER(C.c_int)]
+        lib.mcvd_conv_umma_launch_info.restype = C.c_int
+        lib.mcvd_conv_umma_launch_info.argtypes = [C.POINTER(McvdOp), C.c_int, C.POINTER(C.c_int)]
         lib.mcvd_umma2_stats_bytes.restype = C.c_longlong
         lib.mcvd_umma2_stats_bytes.argtypes = [C.c_int] * 5
         lib.mcvd_umma2_pack_weights.restype = C.c_longlong
@@ -206,6 +208,18 @@ def umma2_plan_info(H, W, ks, c0, c1, c2, c3, n_tile, stats):
     if load().mcvd_umma2_plan_info(H, W, ks, c0, c1, c2, c3, n_tile, 1 if stats else 0, out) != 0:
         return None
     return dict(zip(("kb", "hp", "sa", "r", "nb", "nj", "tmem_cols", "smem", "j", "nsets"), list(out)))
+
+
+LAUNCH_INFO_FIELDS = ("kb", "mt", "sa", "nb", "ra", "npi", "items", "grid", "smem")
+
+
+def conv_umma_launch_info(op: McvdOp, sms: int = 132) -> dict:
+    """the launch plan of a CONV_UMMA / CONV_UMMA2 op on ``sms`` SMs, as the launcher computes it (host arithmetic
+    only): K-block, tile height, slab / weight / raw-input stages, n tiles per work item (> 1: input-stationary),
+    work items, grid and dynamic shared memory bytes.  Raises RuntimeError with the launcher's error text."""
+    out = (C.c_int * len(LAUNCH_INFO_FIELDS))()
+    check(load().mcvd_conv_umma_launch_info(C.byref(op), sms, out), "conv_umma_launch_info")
+    return dict(zip(LAUNCH_INFO_FIELDS, list(out)))
 
 
 def umma2_pick_nt(cout: int, ks: int) -> int:

@@ -66,10 +66,18 @@ def tile_stats(y, ks):
     return st
 
 
+def round_fp16(x):
+    """the half kernel's saturating round-to-nearest fp16 conversion (cvt.rn.satfinite), in x's dtype"""
+    return x.clamp(-65504.0, 65504.0).half().to(x.dtype)
+
+
 class Interpreter:
-    def __init__(self, compute_dtype=torch.float32):
+    def __init__(self, compute_dtype=torch.float32, half=False):
+        """half: emulate MCVD_F_HALF convs -- the transformed activations and the weights after their 2^k pre-scale
+        (mcvd_b200.program.umma_scale_log2 over both K-segments) rounded to fp16 -- instead of ignoring the flag"""
         self.tensors = {}
         self.cdt = compute_dtype
+        self.half = half
 
     # -- registry ---------------------------------------------------------------------------------
     def register(self, t: torch.Tensor):
@@ -118,12 +126,14 @@ class Interpreter:
             a = torch.cat([a, b], dim=3)
         return a
 
-    def _conv(self, op, x, taps_shape_out, mag=False):
+    def _conv(self, op, x, taps_shape_out, mag=False, wround=None):
         """x [B,H,W,Cin] NHWC; weights [taps][Cin][OP]; returns [B,H,W,Cout]"""
         B, H, W, Cin = x.shape
         ks, Cout = op.i0, op.Cout
         OP = taps_shape_out
         w = self.rd(op.w, ks * ks * Cin * OP).view(ks, ks, Cin, OP)[..., :Cout]
+        if wround is not None:
+            w = wround(w)
         if mag:
             w = w.abs()
         wt = w.permute(3, 2, 0, 1).contiguous()                     # OIHW
@@ -291,7 +301,14 @@ class Interpreter:
             else:
                 OP = op.i1
                 scale, wscale = float(op.f0), 1.0
-            y = self._conv(op, m(x), OP, magnitude) * wscale
+            wround = None
+            if self.half and op.flags & lib.F_HALF and not magnitude:
+                from mcvd_b200.program import umma_scale_log2
+                n_all = op.i0 * op.i0 * C * op.Cout + (op.C2 + op.C3) * op.Cout * (1 if op.src2 else 0)
+                kk = umma_scale_log2(float(self.rd(op.w, n_all).abs().max()))
+                wround = lambda v: round_fp16(v * 2.0 ** kk) * 2.0 ** -kk
+                x = round_fp16(x)
+            y = self._conv(op, m(x), OP, magnitude, wround) * wscale
             if k in (lib.OP_CONV_UMMA, lib.OP_CONV_UMMA2) and op.src2:
                 # second K-segment: raw 1x1 conv of (src2|src3); its [1][C2+C3][Cout] weights follow the main ones
                 Hs = H
@@ -302,6 +319,8 @@ class Interpreter:
                 w_all = self.rd(op.w)
                 n_main = op.i0 * op.i0 * C * op.Cout
                 w2 = w_all[n_main:n_main + Cs * op.Cout].view(Cs, op.Cout)
+                if wround is not None:
+                    a2, w2 = round_fp16(a2), wround(w2)
                 y = y + torch.einsum("bhwc,co->bhwo", m(a2), m(w2))
             y = y + m(self.rd(op.bias, op.Cout))
             if op.aux0:

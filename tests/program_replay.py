@@ -14,7 +14,7 @@ Comparisons (``err`` / ``bound`` <= 1 per element; the worst ratio per op kind i
   * conv-epilogue statistics: exact int64 equality with the statistics of the conv's own stored output;
   * every other kind: |out - ref| <= TAU[kind] * A + u * |ref|, with A the op evaluated in float64 on absolute values
     (``Interpreter.exec(magnitude=True)``) and u the unit roundoff of the stored type (2^-23 covers the rounding of
-    both the reference and the kernel to fp32).
+    both the reference and the kernel to fp32); tensor-core convs with MCVD_F_HALF by the one-product model below.
 """
 from __future__ import annotations
 
@@ -25,7 +25,7 @@ import torch
 from mcvd_b200 import lib
 from mcvd_b200.lib import McvdOp
 from mcvd_b200.program import Engine
-from op_interpreter import MAGNITUDE_KINDS, Interpreter, tile_geometry, tile_slots, tile_stats
+from op_interpreter import SILU_LIPSCHITZ, MAGNITUDE_KINDS, Interpreter, tile_geometry, tile_slots, tile_stats
 
 KIND_NAME = {v: k[3:] for k, v in vars(lib).items() if k.startswith("OP_") and isinstance(v, int)}
 
@@ -39,6 +39,15 @@ TAU = {lib.OP_CONV_UMMA: TAU_MATMUL, lib.OP_CONV_UMMA2: TAU_MATMUL, lib.OP_CONV_
        lib.OP_ATTENTION_UMMA: TAU_MATMUL,
        lib.OP_APPLY: 16 * 2.0 ** -24, lib.OP_TIMESTEP_EMBED: 8 * 2.0 ** -24, lib.OP_DIFFUSION_UPDATE: 8 * 2.0 ** -24,
        lib.OP_GN_PARTIAL: 1e-12}
+# Ops with MCVD_F_HALF (model.conv_precision = "fp16") run one fp16 product per term: each operand (the transformed
+# activation, the weight after its 2^k pre-scale) rounds once to fp16, so a term errs by at most (2u + u^2) of its
+# magnitude (u = 2^-11) while both are normal, plus (1 + u) times a subnormal operand's absolute error, 2^-25 for an
+# activation and 2^-25 * 2^-k for a weight, times the other operand:
+#     TAU_HALF * A + u_fp32 |ref| + (1 + u) 2^-25 (sum |w| + 2^-k sum |x|)   (sums over the products)
+# with the fp32 accumulation inside TAU_HALF.  tests/test_conv_fp16_cpu.py checks the model on the CPU.
+U_FP16 = 2.0 ** -11
+TAU_HALF = 2 * U_FP16 + U_FP16 ** 2 + TAU_MATMUL
+HALF_FLOOR = (1 + U_FP16) * 2.0 ** -25
 LAYOUT_KINDS = (lib.OP_NCHW_TO_NHWC, lib.OP_NHWC_TO_NCHW, lib.OP_RESIZE_NEAREST, lib.OP_COPY)
 TC_CONV_KINDS = (lib.OP_CONV_UMMA, lib.OP_CONV_UMMA2)
 PTR_FIELDS = ("src0", "src1", "src2", "src3", "w", "bias", "aux0", "aux1", "aux2", "dst", "dst2")
@@ -118,6 +127,7 @@ class Replay:
         self.stats = {}                  # kind name -> [ops replayed, worst err / bound]
         self.failures = []
         self.range_max = {}              # op label -> max |x| of a statistics-writing conv output
+        self.n_half = 0                  # tensor-core convs judged by the one-product (MCVD_F_HALF) bound
 
     # -- pairing -----------------------------------------------------------------------------------
     def _map(self, where, i, f, rp, tp):
@@ -199,10 +209,34 @@ class Replay:
                 self._record(label, r, f, 0.0 if torch.equal(got, ref[f]) else float("inf"), got, ref[f])
             elif k == lib.OP_GN_FINALIZE:
                 self._check_finalize(label, r, f, got, ref[f])
+            elif k in TC_CONV_KINDS and r.flags & lib.F_HALF:
+                self.n_half += 1
+                bound = TAU_HALF * mag[f].double() + 2.0 ** -23 * ref[f].double().abs() + self._half_floor(r, t)
+                self._ratio(label, r, f, got, ref[f], bound)
             else:
                 u = 2.0 ** -52 if dt == torch.float64 else 2.0 ** -23
                 bound = TAU[k] * mag[f].double() + u * ref[f].double().abs()
                 self._ratio(label, r, f, got, ref[f], bound)
+
+    def _half_floor(self, r, t):
+        """HALF_FLOOR (sum |w| + 2^-k sum |x|) of a half-mode conv, times the output scale and SiLU factor of its
+        magnitude: sum |x| over the products is the magnitude pass with every weight 1 (which adds |bias| and |residual|,
+        a looser bound), sum |w| is bounded by each output channel's sum over all taps and channels; 2^-k is the real
+        op's f1"""
+        w = self.tbuf(t, "w")
+        saved = w.clone()
+        w.fill_(1.0)
+        self._load_inputs(r, t)
+        self.twin.backend.exec(t, magnitude=True)
+        n = r.B * r.H * r.W * r.Cout
+        fx = self.tbuf(t, "dst", n).double().clone()
+        w.copy_(saved)
+        main = r.i0 * r.i0 * (r.C0 + r.C1) * r.Cout
+        wsum = saved[:main].view(-1, r.Cout).abs().double().sum(0)
+        if r.src2:
+            wsum = wsum + saved[main:main + (r.C2 + r.C3) * r.Cout].view(-1, r.Cout).abs().double().sum(0)
+        fw = (wsum * abs(float(r.f0)) * (SILU_LIPSCHITZ if r.flags & lib.F_ACT_OUT else 1.0)).repeat(n // r.Cout)
+        return HALF_FLOOR * (fw + float(r.f1) * fx)
 
     # -- checks ------------------------------------------------------------------------------------
     def _ratio(self, label, r, f, got, ref, bound):
@@ -252,8 +286,10 @@ class Replay:
         s = (f"B={r.B} H={r.H} W={r.W} C0={r.C0} C1={r.C1} C2={r.C2} C3={r.C3} Cout={r.Cout} "
              f"i0..i5={[getattr(r, f'i{i}') for i in range(6)]} flags={r.flags:#x} f0={r.f0:.6g}")
         if r.kind in TC_CONV_KINDS:
-            info = lib.umma2_plan_info(r.H, r.W, r.i0, r.C0, r.C1, r.C2, r.C3, r.i1, bool(r.dst2))
-            s += f" plan={info}"
+            try:
+                s += f" plan={lib.conv_umma_launch_info(r)}"
+            except RuntimeError as e:
+                s += f" plan: {e}"
         return s
 
     def release(self):

@@ -28,13 +28,11 @@ from common import make_module
 from mcvd_b200 import arch, configs, detfill, lib
 from mcvd_b200.model import UNetMore_DDPM
 from mcvd_b200.program import Engine, umma_scale_log2
-from op_interpreter import Interpreter
-from program_replay import TAU_MATMUL
+from op_interpreter import Interpreter, round_fp16 as interp_round_fp16
+from program_replay import TAU_HALF, TAU_MATMUL, U_FP16
 from test_value_ranges_cpu import (CONV_FAMILIES, FP16_MAX, SHORTCUT_FAMILIES, SPLIT_FLOOR, U_FP32, conv_case,
                                    conv_scale_log2, interp_conv, worst_ratio)
 
-U_FP16 = 2.0 ** -11
-TAU_HALF = 2 * U_FP16 + U_FP16 ** 2 + TAU_MATMUL
 
 
 def half_bound(case):
@@ -51,7 +49,7 @@ def half_bound(case):
 
 def round_fp16(x):
     """the kernel's saturating fp16 rounding (cvt.rn.satfinite) as a float64 tensor"""
-    return x.double().clamp(-FP16_MAX, FP16_MAX).half().double()
+    return interp_round_fp16(x.double())
 
 
 def round_bits(x, bits):
@@ -133,6 +131,67 @@ def test_small_prescale_leaves_the_half_bound():
 def test_half_rounding_saturates():
     x = torch.tensor([7e4, -1e6, 65504.0, 1.0 + 2.0 ** -12])
     assert round_fp16(x).tolist() == [65504.0, -65504.0, 65504.0, 1.0]
+
+
+# ------------------------------------------------------------------------------------ rounding offsets on a grid
+# Offsets, in fp16 ulps of a grid value, that tests/test_gpu_conv_half_paths.py adds to the half kernel's operands:
+# +-1/2 is a tie (round-to-nearest-even keeps a grid value, whose significand is even), the others are nearer to it.
+DELTAS = (2.0 ** -2, -2.0 ** -2, 2.0 ** -1 - 2.0 ** -12, -(2.0 ** -1 - 2.0 ** -12), 2.0 ** -1, -2.0 ** -1)
+
+
+def ulp_fp16(v):
+    """the smaller of the fp16 spacings on either side of each normal value of v (float64): below a power of two it
+    is half the spacing above"""
+    m, e = torch.frexp(v.double().abs())
+    u = torch.ldexp(torch.ones_like(m), e - 11)
+    return torch.where(m == 0.5, u / 2, u)
+
+
+def nudge(v, g):
+    """v (float64, normal fp16 values or zero) plus an offset from DELTAS, drawn per element from generator g, times
+    ulp_fp16(v); zeros stay zero"""
+    i = torch.randint(0, len(DELTAS), v.shape, generator=g)
+    d = torch.tensor(DELTAS, dtype=torch.float64)[i]
+    return torch.where(v == 0, v, v + d * ulp_fp16(v))
+
+
+def trunc_fp16(x):
+    """x (float64, fp16 normal range) rounded toward zero to 11 significand bits: a deliberately wrong rounding"""
+    m, e = torch.frexp(x.double())
+    return torch.ldexp(torch.trunc(torch.ldexp(m, torch.full_like(e, 11))), e - 11)
+
+
+def grid_values(n=4096, seed=1):
+    g = torch.Generator().manual_seed(seed)
+    v = torch.randint(-128, 129, (n,), generator=g).double() * 2.0 ** -6
+    w = torch.randint(-4, 5, (n,), generator=g).double() * 2.0 ** 6          # pre-scaled weights (k = 10)
+    return torch.cat([v, w]), g
+
+
+def test_nudged_grid_values_round_back_to_nearest():
+    v, g = grid_values()
+    x = nudge(v, g)
+    assert torch.equal(x.float().double(), x)                              # exact fp32 inputs
+    assert torch.equal(round_fp16(x), v)
+    frac = ((x - v) / ulp_fp16(v))[v != 0]
+    assert set(frac.unique().tolist()) == set(DELTAS)
+    ties = frac.abs() == 0.5
+    assert ties.any() and torch.equal(round_fp16(x)[v != 0][ties], v[v != 0][ties])
+
+
+def test_truncation_is_off_by_one_ulp_where_the_offset_points_to_zero():
+    """the wrong rounding the GPU test rules out: toward zero it lands one ulp below the grid value exactly where the
+    offset's sign is opposite to the value's, and on it elsewhere"""
+    v, g = grid_values(seed=2)
+    x = nudge(v, g)
+    t = trunc_fp16(x)
+    inward = (x.abs() < v.abs())
+    assert inward.any() and (~inward & (v != 0)).any()
+    assert torch.equal(t[~inward], v[~inward])
+    assert torch.equal((v - t)[inward].abs(), ulp_fp16(v)[inward])
+    # an exact-grid conv through the two roundings: the outputs differ
+    xs, ws = x[:64].view(8, 8), torch.ones(8, 8, dtype=torch.float64)
+    assert not torch.equal(round_fp16(xs) @ ws, trunc_fp16(xs) @ ws)
 
 
 # ----------------------------------------------------------------------------------------------------- config key
@@ -259,3 +318,37 @@ def test_modes_never_share_keys(tmp_path):
         e.cache_dir, e.backend = str(tmp_path), None
         paths.append(e._cache_path())
     assert paths[0] and paths[1] and paths[0] != paths[1]
+
+
+# ------------------------------------------------------------------------------------------- tile heights (README)
+# The conv groups (ks, H, Cin, Csc, Cout, n tile) that half mode moves from 128- to 192-position tiles at the benchmark
+# batch on an H100 SXM (132 SMs), as the README's "Half-precision convolutions" section lists them
+HALF_MT192 = {
+    "cfg2": {(3, 64, 192, 0, 192, 192), (3, 64, 192, 192, 192, 192)},
+    "cfg3": {(3, 64, 128, 0, 384, 192)},
+    "cfg4": {(3, 64, 32, 0, 192, 192), (3, 64, 192, 0, 192, 192), (3, 64, 192, 384, 192, 192),
+             (3, 64, 192, 576, 192, 192), (3, 64, 384, 0, 192, 192), (3, 64, 384, 0, 384, 192),
+             (3, 64, 384, 384, 384, 192), (3, 64, 576, 0, 192, 192)},
+    "cfg5": {(3, 64, 384, 0, 384, 192), (3, 64, 384, 384, 384, 192)},
+}
+
+
+@pytest.mark.parametrize("name", sorted(HALF_MT192))
+def test_half_mode_tile_heights_match_the_readme(name):
+    """every tensor-core conv of the lowered forward keeps its tile height in half mode except the README's groups,
+    which go from 128 to 192 positions (the launcher's own plan, mcvd_conv_umma_launch_info, at 132 SMs)"""
+    heights = {}
+    for precision in ("fp32", "fp16"):
+        cfg = configs.workload(name)
+        cfg.model.conv_precision = precision
+        cfg, net, sd = make_module(cfg, "cpu")
+        eng = Engine(net, _test_backend=Interpreter())
+        P = eng.program(cfg.bench_batch)
+        heights[precision] = [((o.i0, o.H, o.C0 + o.C1, o.C2 + o.C3, o.Cout, o.i1), lib.conv_umma_launch_info(o, 132)["mt"])
+                              for o in P.step_ops + P.cond_ops if o.kind in (lib.OP_CONV_UMMA, lib.OP_CONV_UMMA2)]
+        del P, eng, net
+    assert [g for g, _ in heights["fp32"]] == [g for g, _ in heights["fp16"]]
+    changed = {g32 for (g32, m32), (_, m16) in zip(heights["fp32"], heights["fp16"]) if m32 != m16}
+    assert changed == HALF_MT192[name]
+    assert all(m32 == 128 and m16 == 192 for (g, m32), (_, m16) in zip(heights["fp32"], heights["fp16"])
+               if g in changed)

@@ -25,6 +25,7 @@ from common import golden, make_module, step_noise
 from mcvd_b200 import configs, detfill, lib, runner, samplers
 from oracle import gen_golden_gamma as GG, mcvd_oracle as O
 from test_conv_fp16_cpu import half_bound
+import test_gpu_conv2 as C2
 from test_gpu_value_ranges import stressed_state_dict
 from test_value_ranges_cpu import CONV_FAMILIES, SHORTCUT_FAMILIES, conv_case, conv_op, worst_ratio
 
@@ -57,46 +58,69 @@ def packer():
 
 # ---------------------------------------------------------------------------------------------------------- op level
 HALF_SHAPES = [
-    # B, H, C0, C1, Cout, ks, C2, i2 (work organisation), tab, res, tile heights
-    (2, 16, 64, 0, 96, 3, 0, 1, True, True, (128, 192)),      # streaming 3x3, fused norm, residual
-    (3, 8, 32, 32, 64, 3, 0, 1, False, False, (128, 192)),    # virtual concat
-    (2, 16, 96, 0, 192, 1, 0, 1, True, False, (128, 192)),    # 1x1 streaming
-    (4, 8, 64, 0, 64, 1, 0, 2, False, True, (128,)),          # 1x1 input-stationary
-    (2, 16, 64, 0, 64, 3, 32, 1, True, False, (128, 192)),    # fused 1x1 shortcut
-    (2, 8, 48, 48, 96, 3, 0, 1, False, True, (128, 192)),     # K-block 16
+    # B, H, C0, C1, Cout, ks, C2, i2 (work organisation), tab, res, tile heights, extra (n tile, i5, act_out, planar:
+    # CONV_UMMA2 with the planar table and epilogue statistics)
+    (2, 16, 64, 0, 96, 3, 0, 1, True, True, (128, 192), {}),      # streaming 3x3, fused norm, residual
+    (3, 8, 32, 32, 64, 3, 0, 1, False, False, (128, 192), {}),    # virtual concat
+    (2, 16, 96, 0, 192, 1, 0, 1, True, False, (128, 192), {}),    # 1x1 streaming
+    (4, 8, 64, 0, 192, 1, 0, 2, False, True, (128,), dict(nt=64)),     # 1x1 input-stationary: three n tiles per item
+    (2, 16, 64, 0, 64, 3, 32, 1, True, False, (128, 192), {}),    # fused 1x1 shortcut
+    (2, 8, 48, 48, 96, 3, 0, 1, False, True, (128, 192), {}),     # K-block 16
+    (2, 16, 64, 0, 96, 3, 0, 1, True, False, (128, 192), dict(act_out=True)),     # output SiLU
+    (1, 128, 32, 0, 96, 3, 0, 1, True, False, (192,), dict(i5=3)),     # three slab stages at 128x128: half mode only
+    (2, 16, 64, 0, 144, 3, 0, 1, True, True, (128, 192), dict(nt=144)),          # n tile 144
+    (2, 8, 64, 0, 384, 3, 0, 1, True, False, (128, 192), dict(nt=192)),          # two n tiles
+    (2, 16, 64, 0, 64, 3, 32, 0, True, False, (128,), dict(planar=True)),        # planar table, statistics
 ]
 
 
-def run_half(packer, case, nacc, mt):
+def run_half(packer, case, nacc, mt, extra):
     B, H, W, C0 = case["x0"].shape
     C1 = 0 if case.get("x1") is None else case["x1"].shape[3]
     Cout = case["taps"].shape[2]
     taps, sc = case["taps"], case.get("taps_sc")
-    nt = max(d for d in range(16, 257, 16) if Cout % d == 0)
+    nt = extra.get("nt") or max(d for d in range(16, 257, 16) if Cout % d == 0)
     kb = lib.umma_kblock(C0, C1)
     w, f1 = packer._pack_umma(taps, nt, kb, True) if sc is None else packer._pack_umma_fused(taps, sc, nt, kb, True)
     assert w.numel() == 2 * (taps.numel() + (0 if sc is None else sc.numel()))        # hi only: 2 bytes a weight
     dst = torch.full((B, H, W, Cout), float("nan"), device=DEV)
-    op = conv_op(case, lib.OP_CONV_UMMA, w, f1, dst)
-    op.i1, op.i2, op.i4, op.flags = nt, nacc, mt, op.flags | lib.F_HALF
+    st = None
+    if extra.get("planar"):
+        st = torch.full((lib.umma2_stats_bytes(B, H, W, case["ks"], Cout) // 8,), -7, dtype=torch.int64, device=DEV)
+        tab3 = C2.planar(case["tab"]).contiguous()
+        op = conv_op(case, lib.OP_CONV_UMMA2, w, f1, dst, tab=tab3)
+        op.dst2, op.i2 = st.data_ptr(), kb
+    else:
+        op = conv_op(case, lib.OP_CONV_UMMA, w, f1, dst)
+        op.i2, op.i4, op.i5 = nacc, mt, extra.get("i5", 0)
+    op.i1, op.flags = nt, op.flags | lib.F_HALF
     run(op)
-    return dst
+    torch.cuda.synchronize()
+    return dst, st
 
 
-@pytest.mark.parametrize("shape", HALF_SHAPES, ids=lambda s: "B{}H{}C{}+{}-{}k{}sc{}n{}".format(*s[:8]))
+@pytest.mark.parametrize("shape", HALF_SHAPES,
+                         ids=lambda s: "B{}H{}C{}+{}-{}k{}sc{}n{}".format(*s[:8]) + "".join(f"-{k}{v}" for k, v in s[11].items()))
 def test_half_conv_meets_the_one_product_bound(packer, shape):
-    B, H, C0, C1, Cout, ks, C2, nacc, tab, res, heights = shape
+    B, H, C0, C1, Cout, ks, C2_, nacc, tab, res, heights, extra = shape
     report = []
-    for fam in CONV_FAMILIES + (SHORTCUT_FAMILIES if C2 else ()):
-        case = conv_case(fam, B, H, C0, Cout, ks, C1=C1, C2=C2, tab=tab, res=res)
+    stats_checked = 0
+    for fam in CONV_FAMILIES + (SHORTCUT_FAMILIES if C2_ else ()):
+        case = conv_case(fam, B, H, C0, Cout, ks, C1=C1, C2=C2_, tab=tab, res=res, act_out=extra.get("act_out", False))
         case = {k: v.to(DEV) if isinstance(v, torch.Tensor) else v for k, v in case.items()}
         ref, bound = half_bound(case)
-        outs = [run_half(packer, case, nacc, mt) for mt in heights]
-        for o in outs[1:]:
-            assert torch.equal(o, outs[0]), f"{fam}: MT = {heights} differ"
-        report.append((fam, worst_ratio(outs[0], ref, bound)))
+        outs = [run_half(packer, case, nacc, mt, extra) for mt in heights]
+        for o, _ in outs[1:]:
+            assert torch.equal(o, outs[0][0]), f"{fam}: MT = {heights} differ"
+        out, st = outs[0]
+        if st is not None and float(out.abs().max()) <= 4096.0:       # the statistics' documented range
+            exp = C2.expected_stats(out.cpu(), ks)
+            assert torch.equal(st.cpu().view(exp.shape), exp), fam
+            stats_checked += 1
+        report.append((fam, worst_ratio(out, ref, bound)))
     print(f"\n{shape}: worst err/bound " + ", ".join(f"{f} {r:.3g}" for f, r in report))
     assert all(r <= 1.0 for _, r in report), report
+    assert not extra.get("planar") or stats_checked >= 3
 
 
 def test_half_flag_rejects_a_split_experiment(packer):
@@ -147,13 +171,20 @@ def errors(out, ref):
     return float(d.abs().max()) / s, float(d.pow(2).mean().sqrt()) / s
 
 
-NET_ROWS = [(n, v) for n in ("tiny", "tiny_spade", "tiny_rgb", "cfg2") for v in ("trained", "fresh")]
+NET_ROWS = [(n, v, "umma") for n in ("tiny", "tiny_spade", "tiny_rgb", "cfg2") for v in ("trained", "fresh")] + \
+    [("cfg2", "trained", "umma2"), ("cfg2", "trained", "umma+stats")]
 
 
-@pytest.mark.parametrize("name,variant", NET_ROWS, ids=["-".join(r) for r in NET_ROWS])
-def test_network_error_within_twice_the_references_tf32(name, variant):
+@pytest.mark.parametrize("name,variant,mode", NET_ROWS,
+                         ids=["-".join(r[:2]) + ("" if r[2] == "umma" else "-" + r[2]) for r in NET_ROWS])
+def test_network_error_within_twice_the_references_tf32(name, variant, mode):
+    """mode: the lowering's conv mode, umma2 (planar-table convs) or umma+stats (GroupNorm statistics from the conv
+    epilogue) besides the default"""
     torch.set_num_threads(min(torch.get_num_threads(), 16))
     cfg, net16, sd = half_module(name, "fp16", variant=variant)
+    eng = net16.engine()
+    eng.conv_mode = mode.split("+")[0]
+    eng.epilogue_stats = mode in ("umma2", "umma+stats")
     _, net32, _ = half_module(name, "fp32", variant=variant)
     B = 1 if name == "cfg2" else 2
     x, cond = detfill.synthetic_inputs(cfg, B, seed=5)
@@ -171,6 +202,8 @@ def test_network_error_within_twice_the_references_tf32(name, variant):
     assert e32[0] <= max(0.05 * etf[0], 4 * U32 * peak) and e32[1] <= max(0.05 * etf[1], 4 * U32)
     P = net16.engine().program(B)
     assert any(o.flags & lib.F_HALF for o in P.step_ops)
+    if mode != "umma":
+        assert any(o.flags & lib.F_HALF and o.dst2 for o in P.step_ops)       # half convs with epilogue statistics
 
 
 # ----------------------------------------------------------------------------------------------------- samplers

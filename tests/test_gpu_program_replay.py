@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from common import make_module
-from mcvd_b200 import detfill
+from mcvd_b200 import configs, detfill, lib
 from mcvd_b200.program import Engine
 from program_replay import TC_CONV_KINDS, KIND_NAME, replay_program, twin_engine
 
@@ -19,14 +19,16 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 
-def replay_row(name, mode, per_clip_t=False, split_mode=3):
+def replay_row(name, mode, per_clip_t=False, split_mode=3, precision="fp32"):
     """mode: umma | umma+stats (GroupNorm partial sums from the conv epilogue) | umma2 | simt (CUDA-core convs and
-    attention)"""
+    attention); precision: model.conv_precision (fp16: the nn.Conv2d layers' convs carry MCVD_F_HALF)"""
     gc.collect()
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
     t0 = time.perf_counter()
-    cfg, net, _ = make_module(name, DEV)
+    cfg = configs.workload(name)
+    cfg.model.conv_precision = precision
+    cfg, net, _ = make_module(cfg, DEV)
     real = Engine(net)
     real.conv_mode = mode.split("+")[0]
     real.epilogue_stats = mode in ("umma2", "umma+stats")
@@ -44,7 +46,7 @@ def replay_row(name, mode, per_clip_t=False, split_mode=3):
     R.wall_s = time.perf_counter() - t0
     R.peak_gb = torch.cuda.max_memory_allocated() / 2 ** 30
     torch.cuda.empty_cache()
-    print(f"\n{name} B={B} {mode} {'per-clip' if per_clip_t else 'uniform'} t, split {split_mode}: {R.n_ops} ops, "
+    print(f"\n{name} B={B} {mode} {precision} {'per-clip' if per_clip_t else 'uniform'} t, split {split_mode}: {R.n_ops} ops, "
           f"{R.wall_s:.1f} s, peak {R.peak_gb:.1f} GiB, all clips\n{R.table()}")
     if R.range_max:
         print(f"  largest |x| of a statistics-writing conv output: {max(R.range_max.values()):.4g}")
@@ -52,22 +54,31 @@ def replay_row(name, mode, per_clip_t=False, split_mode=3):
 
 
 ROWS = [
-    ("cfg1", "umma", False),
-    ("cfg1", "simt", False),
-    ("cfg2", "umma", False),
-    ("cfg2", "umma", True),            # per-clip t: batched LINEAR, FiLM stride film_total
-    ("cfg2", "umma2", False),
-    ("cfg2", "umma+stats", False),
-    ("cfg3", "umma", False),           # SPADE cond_ops
-    ("cfg4", "umma", False),           # head dim 192, key tile 32, 3 channels
-    ("cfg5", "umma", False),           # 128x128 maps, one-raw-stage plans, 32x32 attention
+    ("cfg1", "umma", False, "fp32"),
+    ("cfg1", "simt", False, "fp32"),
+    ("cfg2", "umma", False, "fp32"),
+    ("cfg2", "umma", True, "fp32"),            # per-clip t: batched LINEAR, FiLM stride film_total
+    ("cfg2", "umma2", False, "fp32"),
+    ("cfg2", "umma+stats", False, "fp32"),
+    ("cfg3", "umma", False, "fp32"),           # SPADE cond_ops
+    ("cfg4", "umma", False, "fp32"),           # head dim 192, key tile 32, 3 channels
+    ("cfg5", "umma", False, "fp32"),           # 128x128 maps, one-raw-stage plans, 32x32 attention
+    # model.conv_precision = fp16: the nn.Conv2d layers' convs by the one-product bound, their statistics exact
+    ("cfg1", "umma", False, "fp16"),
+    ("cfg2", "umma", False, "fp16"),
+    ("cfg2", "umma2", False, "fp16"),
+    ("cfg2", "umma+stats", False, "fp16"),
+    ("cfg3", "umma", False, "fp16"),
+    ("cfg4", "umma", False, "fp16"),
+    ("cfg5", "umma", False, "fp16"),
 ]
 
 
-@pytest.mark.parametrize("name,mode,per_clip_t", ROWS,
-                         ids=[f"{n}-{m}-{'perclip' if p else 'uniform'}" for n, m, p in ROWS])
-def test_program_replay(name, mode, per_clip_t):
-    R = replay_row(name, mode, per_clip_t)
+@pytest.mark.parametrize("name,mode,per_clip_t,precision", ROWS,
+                         ids=[f"{n}-{m}-{'perclip' if p else 'uniform'}" + ("" if c == "fp32" else "-" + c)
+                              for n, m, p, c in ROWS])
+def test_program_replay(name, mode, per_clip_t, precision):
+    R = replay_row(name, mode, per_clip_t, precision=precision)
     assert not R.failures, f"{len(R.failures)} outputs over their bound:\n" + "\n".join(R.failures[:20])
     assert R.whole_program_identical, "op-by-op eps differs from one run of the whole program"
     kinds = {k.split(".")[0] for k in R.stats}
@@ -81,6 +92,7 @@ def test_program_replay(name, mode, per_clip_t):
         assert R.range_max and max(R.range_max.values()) <= 4096.0
     if name == "cfg3":
         assert "RESIZE_NEAREST" in kinds
+    assert (R.n_half > 0) == (precision == "fp16")
 
 
 @pytest.mark.parametrize("name", ["cfg1", "cfg2"])

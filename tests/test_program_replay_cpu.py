@@ -5,15 +5,17 @@ import pytest
 import torch
 
 from common import make_module
-from mcvd_b200 import detfill, lib
+from mcvd_b200 import configs, detfill, lib
 from mcvd_b200.program import Engine
 from op_interpreter import Interpreter, tile_stats
 from program_replay import HarnessError, Replay, replay_program, twin_engine
 
 
-def cpu_pair(name, conv_mode, epilogue_stats=False):
-    cfg, net, _ = make_module(name, "cpu")
-    real = Engine(net, _test_backend=Interpreter())
+def cpu_pair(name, conv_mode, epilogue_stats=False, precision="fp32"):
+    cfg = configs.workload(name)
+    cfg.model.conv_precision = precision
+    cfg, net, _ = make_module(cfg, "cpu")
+    real = Engine(net, _test_backend=Interpreter(half=precision == "fp16"))
     real.conv_mode, real.epilogue_stats = conv_mode, epilogue_stats
     return cfg, net, real, twin_engine(real, net)
 
@@ -77,3 +79,32 @@ def test_epilogue_statistics_range_is_enforced():
         y[1, 3, 4, 5] = bad
         with pytest.raises(ValueError):
             tile_stats(y, 3)
+
+
+@pytest.mark.parametrize("name,conv_mode,stats", [("tiny", "umma", False), ("tiny_spade", "umma", False),
+                                                  ("tiny", "umma2", True)])
+def test_half_emulation_replays_within_the_one_product_bound(name, conv_mode, stats):
+    """the interpreter's fp16 emulation of MCVD_F_HALF convs (operands rounded once to fp16) replayed against the
+    float64 twin: inside the one-product bound, statistics exact"""
+    cfg, net, real, twin = cpu_pair(name, conv_mode, stats, precision="fp16")
+    B = cfg.bench_batch
+    x, cond = detfill.synthetic_inputs(cfg, B)
+    R = replay_program(real, twin, B, x, cond, 321.0, detfill.normal("replay_z", x.shape))
+    assert not R.failures, "\n".join(R.failures[:10])
+    assert R.n_half > 0
+    if stats:
+        assert R.stats["CONV_UMMA2.dst2"][0] > 0
+    # the half rounding is visible: a worst ratio far above the default mode's TAU_MATMUL-sized errors
+    assert max(w for k, (n, w) in R.stats.items() if k.startswith("CONV_UMMA")) > 0.01, R.table()
+
+
+def test_replay_flags_a_wrong_half_op():
+    """one half-mode conv whose weights are scaled by 1 + 2^-4 is reported on that op and no other"""
+    cfg, net, real, twin = cpu_pair("tiny", "umma", precision="fp16")
+    B = cfg.bench_batch
+    P = real.program(B)
+    i = next(j for j, o in enumerate(P.step_ops) if o.kind == lib.OP_CONV_UMMA and o.flags & lib.F_HALF and j > 10)
+    real.backend.tensors[P.step_ops[i].w].mul_(1 + 2.0 ** -4)
+    x, cond = detfill.synthetic_inputs(cfg, B)
+    R = replay_program(real, twin, B, x, cond, 500.0, detfill.normal("replay_z", x.shape))
+    assert R.failures and all(f.startswith(f"step[{i}] CONV_UMMA") for f in R.failures), R.failures[:3]
