@@ -269,6 +269,14 @@ enum {
    * mcvd_tf32_pack_weights(w, K = i0 * i1 * C0, Cout, ...).  The fused pool is formed in fp32 and rounded once.
    * Numerics as MCVD_OP_CONV3D_TF32. */
   MCVD_OP_CONV2D_TF32 = 35,
+  /* Not a kind: 36 is left unassigned and is rejected as an unknown kind, as it was when 35 was the last kind;
+   * existing callers and tests (tests/test_eval_tf32_cpu.py) rely on that. */
+  MCVD_OP__UNASSIGNED_36 = 36,
+  /* MCVD_OP_CONV_RELU on the TF32 tensor cores: every field, the MCVD_F_POOL flag and the geometry contract are
+   * MCVD_OP_CONV_RELU's, except w: the packed TF32 image of the [i0][i0][C0][Cout] weights,
+   * mcvd_tf32_pack_weights(w, K = i0 * i0 * C0, Cout, ...).  The max-pool on read is formed in fp32 and rounded once.
+   * Numerics as MCVD_OP_CONV3D_TF32: a frame pair's distance does not depend on the batch or chunk it is in. */
+  MCVD_OP_CONV_RELU_TF32 = 37,
   MCVD_OP__COUNT
 };
 
@@ -372,8 +380,9 @@ long long mcvd_umma2_stats_bytes(int B, int H, int W, int ks, int Cout);
  * this call fills (taps*Cin*Cout*4); out == NULL only queries. */
 long long mcvd_umma2_pack_weights(const float* w_taps, int taps, int Cin, int Cout, int n_tile, int k_block,
                                   void* out, int scale_log2, int stage_off, int per_unit, void* stream);
-/* Packed TF32 weights of MCVD_OP_CONV3D_TF32 / MCVD_OP_CONV2D_TF32.  w_kmajor = fp32 [K][Cout] on the device (the
- * MCVD_OP_CONV3D / MCVD_OP_CONV2D layout; K = taps * Cin, Cout a positive multiple of 8); out = device buffer of
+/* Packed TF32 weights of MCVD_OP_CONV3D_TF32 / MCVD_OP_CONV2D_TF32 / MCVD_OP_CONV_RELU_TF32.  w_kmajor = fp32
+ * [K][Cout] on the device (the MCVD_OP_CONV3D / MCVD_OP_CONV2D / MCVD_OP_CONV_RELU layout; K = taps * Cin, Cout a
+ * positive multiple of 8); out = device buffer of
  * mcvd_tf32_packed_bytes(K, Cout) bytes, 16-byte aligned, written on `stream`.  Every value is rounded to TF32
  * (round to nearest, ties away from zero); the layout (n tiles and K slabs padded with zeros) belongs to the library.
  * mcvd_tf32_packed_bytes returns < 0 for an unusable K / Cout; mcvd_tf32_pack_weights returns 0 or < 0. */

@@ -42,7 +42,8 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
     case MCVD_OP_MAXPOOL3D:
     case MCVD_OP_MAXPOOL2D: return launch_maxpool(op, s);
     case MCVD_OP_CONV3D_TF32:
-    case MCVD_OP_CONV2D_TF32: return launch_conv_tf32(op, s);
+    case MCVD_OP_CONV2D_TF32:
+    case MCVD_OP_CONV_RELU_TF32: return launch_conv_tf32(op, s);
     case MCVD_OP_LPIPS_LAYER: return launch_lpips_layer(op, s);
     case MCVD_OP_I3D_PREP: return launch_i3d_prep(op, s);
     case MCVD_OP_I3D_HEAD: return launch_i3d_head(op, s);
@@ -59,7 +60,7 @@ static int dispatch(const McvdOp& op, cudaStream_t s) {
 }
 
 static int validate_one(const McvdOp& op, int idx) {
-  if (op.kind <= 0 || op.kind >= MCVD_OP__COUNT) {
+  if (op.kind <= 0 || op.kind >= MCVD_OP__COUNT || op.kind == MCVD_OP__UNASSIGNED_36) {
     set_error("op %d: unknown kind %d", idx, op.kind);
     return -1;
   }
@@ -153,9 +154,11 @@ static int validate_one(const McvdOp& op, int idx) {
     case MCVD_OP_CONV2D:
     case MCVD_OP_MAXPOOL2D:
     case MCVD_OP_CONV3D_TF32:
-    case MCVD_OP_CONV2D_TF32: {
+    case MCVD_OP_CONV2D_TF32:
+    case MCVD_OP_CONV_RELU_TF32: {
       ConvGeom g;
-      const bool tf32 = op.kind == MCVD_OP_CONV3D_TF32 || op.kind == MCVD_OP_CONV2D_TF32;
+      const bool tf32 = op.kind == MCVD_OP_CONV3D_TF32 || op.kind == MCVD_OP_CONV2D_TF32 ||
+                        op.kind == MCVD_OP_CONV_RELU_TF32;
       if (const char* why = tf32 ? conv_tf32_geom(op, g) : conv_geom(op, g)) {
         set_error("op %d %s: %s", idx, conv_kind_name(op.kind), why);
         return -1;

@@ -266,7 +266,8 @@ static const char* maxpool2d_geom(const McvdOp& op, ConvGeom& g) {
 
 const char* conv_geom(const McvdOp& op, ConvGeom& g) {
   switch (op.kind) {
-    case MCVD_OP_CONV_RELU: return conv_relu_geom(op, g);
+    case MCVD_OP_CONV_RELU:
+    case MCVD_OP_CONV_RELU_TF32: return conv_relu_geom(op, g);
     case MCVD_OP_CONV3D:
     case MCVD_OP_CONV3D_TF32: return conv3d_geom(op, g);
     case MCVD_OP_MAXPOOL3D: return maxpool3d_geom(op, g);
@@ -279,7 +280,8 @@ const char* conv_geom(const McvdOp& op, ConvGeom& g) {
 
 int gather_mode(const McvdOp& op) {
   switch (op.kind) {
-    case MCVD_OP_CONV_RELU: return (op.flags & MCVD_F_POOL) ? G_S2MAX : G_CONV2;
+    case MCVD_OP_CONV_RELU:
+    case MCVD_OP_CONV_RELU_TF32: return (op.flags & MCVD_F_POOL) ? G_S2MAX : G_CONV2;
     case MCVD_OP_CONV3D:
     case MCVD_OP_CONV3D_TF32: return op.i0 == 1 && op.i1 == 1 && op.i2 == 1 && op.i3 == 1 ? G_PW : G_CONV3;
     default:
@@ -297,6 +299,7 @@ const char* conv_kind_name(int kind) {
     case MCVD_OP_MAXPOOL2D: return "MAXPOOL2D";
     case MCVD_OP_CONV3D_TF32: return "CONV3D_TF32";
     case MCVD_OP_CONV2D_TF32: return "CONV2D_TF32";
+    case MCVD_OP_CONV_RELU_TF32: return "CONV_RELU_TF32";
     default: return "?";
   }
 }

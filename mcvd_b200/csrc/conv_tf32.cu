@@ -1,7 +1,7 @@
-// TF32 tensor-core convolutions of the FVD (I3D) and FID (Inception-v3) feature networks: MCVD_OP_CONV3D_TF32 and
-// MCVD_OP_CONV2D_TF32 in include/mcvd_b200.h.  Same geometry, gather, epilogue and channel-slice output as
-// MCVD_OP_CONV3D and MCVD_OP_CONV2D (conv_eval.cuh, conv_eval.cu); the products run on wgmma m64nNk8 tf32 with fp32
-// accumulators.
+// TF32 tensor-core convolutions of the FVD (I3D), FID (Inception-v3) and LPIPS (AlexNet) networks:
+// MCVD_OP_CONV3D_TF32, MCVD_OP_CONV2D_TF32 and MCVD_OP_CONV_RELU_TF32 in include/mcvd_b200.h.  Same geometry, gather,
+// epilogue and channel-slice output as MCVD_OP_CONV3D, MCVD_OP_CONV2D and MCVD_OP_CONV_RELU (conv_eval.cuh,
+// conv_eval.cu); the products run on wgmma m64nNk8 tf32 with fp32 accumulators.
 //
 // Implicit GEMM: M = output positions (video * t * y * x, or frame * y * x), N = Cout, K = taps * Cin in
 // (dt, dy, dx, c) order.  A CTA of two warpgroups computes a 128-position x BN tile; K advances in slabs of 32.
@@ -210,14 +210,18 @@ static int run_tf32_mode(const McvdOp& op, const ConvGeom& g, cudaStream_t s) {
 }
 
 int launch_conv_tf32(const McvdOp& op, cudaStream_t s) {
+  // the AlexNet geometry leaves the input and output pointers to this check, as launch_conv_ffma does
+  if (op.kind == MCVD_OP_CONV_RELU_TF32) MCVD_CHECK(op.src0 && op.dst, "%s: null pointer", conv_kind_name(op.kind));
   ConvGeom g;
   if (const char* why = conv_tf32_geom(op, g)) MCVD_CHECK(false, "%s: %s", conv_kind_name(op.kind), why);
+  // G_S2MAX keeps its 3x3 window unrolled: at 128 registers it still fits two CTAs per SM without spilling
   switch (gather_mode(op)) {
     case G_CONV2: return run_tf32_mode<G_CONV2>(op, g, s);
     case G_CONV3: return run_tf32_mode<G_CONV3>(op, g, s);
     case G_PW: return run_tf32_mode<G_PW>(op, g, s);
     case G_BMAX: return run_tf32_mode<G_BMAX>(op, g, s);
-    default: return run_tf32_mode<G_BAVG>(op, g, s);
+    case G_BAVG: return run_tf32_mode<G_BAVG>(op, g, s);
+    default: return run_tf32_mode<G_S2MAX>(op, g, s);
   }
 }
 

@@ -72,7 +72,7 @@ int launch_fid_head(const McvdOp& op, cudaStream_t s);
 int launch_knn(const McvdOp& op, cudaStream_t s);
 int launch_conv_ffma(const McvdOp& op, cudaStream_t s);   // CONV_RELU, CONV3D, CONV2D (conv_eval.cu)
 int launch_maxpool(const McvdOp& op, cudaStream_t s);     // MAXPOOL3D, MAXPOOL2D (conv_eval.cu)
-int launch_conv_tf32(const McvdOp& op, cudaStream_t s);   // CONV3D_TF32, CONV2D_TF32 (conv_tf32.cu)
+int launch_conv_tf32(const McvdOp& op, cudaStream_t s);   // CONV3D_TF32, CONV2D_TF32, CONV_RELU_TF32 (conv_tf32.cu)
 
 // NULL, or why an op of the I3D kinds is unusable (shared by validation and launch; i3d.cu)
 const char* i3d_prep_error(const McvdOp& op);

@@ -47,6 +47,8 @@ OP_KNN_RADIUS = 32
 OP_KNN_COVER = 33
 OP_CONV3D_TF32 = 34
 OP_CONV2D_TF32 = 35
+OP__UNASSIGNED_36 = 36                  # not a kind: rejected as unknown
+OP_CONV_RELU_TF32 = 37
 
 F_ACT_IN = 1 << 0
 F_ACT_OUT = 1 << 1
@@ -235,8 +237,8 @@ def umma2_pick_nt(cout: int, ks: int) -> int:
 
 
 def tf32_packed_bytes(K: int, cout: int) -> int:
-    """bytes of the packed TF32 weight image of a [K, Cout] convolution (OP_CONV3D_TF32 / OP_CONV2D_TF32); host
-    arithmetic only"""
+    """bytes of the packed TF32 weight image of a [K, Cout] convolution (OP_CONV3D_TF32 / OP_CONV2D_TF32 /
+    OP_CONV_RELU_TF32); host arithmetic only"""
     n = int(load().mcvd_tf32_packed_bytes(K, cout))
     if n < 0:
         raise RuntimeError(f"mcvd_b200 tf32_packed_bytes failed: {last_error()}")
@@ -244,8 +246,8 @@ def tf32_packed_bytes(K: int, cout: int) -> int:
 
 
 def tf32_pack_weights(w):
-    """The packed TF32 image (``w`` of OP_CONV3D_TF32 / OP_CONV2D_TF32) of folded weights ``w`` fp32 [K, Cout] on a
-    CUDA device, as an fp32 tensor on the same device.  The layout belongs to the library."""
+    """The packed TF32 image (``w`` of OP_CONV3D_TF32 / OP_CONV2D_TF32 / OP_CONV_RELU_TF32) of folded weights ``w``
+    fp32 [K, Cout] on a CUDA device, as an fp32 tensor on the same device.  The layout belongs to the library."""
     import torch
     if w.device.type != "cuda" or w.dtype != torch.float32 or w.dim() != 2:
         raise ValueError(f"tf32_pack_weights: weights must be fp32 [K, Cout] on CUDA, got {w.dtype} "

@@ -4,7 +4,9 @@ MCVD's ``video_gen`` reports LPIPS next to MSE, PSNR and SSIM (reference runners
 1602-1609): per frame pair it makes two PIL images, resizes them to 128x128, runs ``PerceptualLoss(model='net-lin',
 net='alex')`` at batch size 1 and sums the distances.  ``LPIPS`` computes the same per-frame distances for whole
 batches with the library's own kernels (``MCVD_OP_LPIPS_PREP``, ``MCVD_OP_CONV_RELU``, ``MCVD_OP_LPIPS_LAYER``):
-11 launches per chunk of frame pairs.
+11 launches per chunk of frame pairs.  ``LPIPS(..., tf32=True)`` runs the five convolutions on the TF32 tensor cores
+instead (``MCVD_OP_CONV_RELU_TF32``): both operands rounded once to TF32, fp32 accumulation, the numerics class of
+cuDNN with ``allow_tf32``.
 
 Weights are never downloaded.  ``LPIPS`` takes either
   * a torchvision AlexNet state_dict (``features.{0,3,6,8,10}.{weight,bias}``, e.g. the torch hub cache's
@@ -92,15 +94,28 @@ class LPIPS:
     current CUDA device).  Frame pairs are processed in chunks of at most ``max_chunk_frames``; a chunk needs
     ``(128*128*4 + 31*31*64) * 4 * 2`` bytes (0.97 MiB) of workspace per frame pair, so the default of 256 pairs
     bounds it at 248 MiB.
+
+    ``tf32``: run the five convolutions on the TF32 tensor cores (``MCVD_OP_CONV_RELU_TF32``).  Activations (after
+    the max-pool of layers 2 and 3) and weights are rounded once to TF32 (round to nearest, ties away from zero) and
+    the products summed in fp32, so the distances differ from the default fp32 ones by about the TF32 rounding
+    (cuDNN's ``allow_tf32`` class of numerics); a frame pair's distance still does not depend on its batch or chunk.
+    The packed TF32 weights are made once here and take 9.9 MB of device memory on top of the 9.9 MB of fp32
+    weights; the workspace and the 11 launches per chunk are unchanged.  The default (False) is the fp32 FFMA path,
+    unchanged.
     """
 
     def __init__(self, backbone, lin=None, device: Optional[Union[str, torch.device]] = None,
-                 max_chunk_frames: int = 256):
+                 max_chunk_frames: int = 256, tf32: bool = False):
         if not 1 <= int(max_chunk_frames) <= 32767:
             raise ValueError(f"LPIPS: max_chunk_frames={max_chunk_frames} must be in [1, 32767]")
         self.device = torch.device(device if device is not None else "cuda")
         self.max_chunk_frames = int(max_chunk_frames)
         self.weights = [tuple(t.to(self.device) for t in layer) for layer in pack_weights(backbone, lin)]
+        self.tf32 = bool(tf32)
+        self.packed: List[torch.Tensor] = []
+        if self.tf32:
+            from . import lib
+            self.packed = [lib.tf32_pack_weights(w) for w, _, _ in self.weights]
         self._tables: Dict[int, torch.Tensor] = {}
 
     def _table(self, size: int) -> torch.Tensor:
@@ -123,10 +138,13 @@ class LPIPS:
         src, dst, side, cin = A, B, SIDE, 4
         for li, (_, _, cout, k, stride, pad, pool) in enumerate(LAYERS):
             w, b, lw = self.weights[li]
+            if self.tf32:
+                w = self.packed[li]
             hc = (side - 3) // 2 + 1 if pool else side
             oh = (hc + 2 * pad - k) // stride + 1
             op = lib.McvdOp()
-            op.kind, op.flags, op.B, op.H, op.W, op.C0, op.Cout = (lib.OP_CONV_RELU, lib.F_POOL if pool else 0, 2 * n,
+            op.kind, op.flags, op.B, op.H, op.W, op.C0, op.Cout = (lib.OP_CONV_RELU_TF32 if self.tf32 else
+                                                                   lib.OP_CONV_RELU, lib.F_POOL if pool else 0, 2 * n,
                                                                    oh, oh, cin, cout)
             op.i0, op.i1, op.i2, op.i3, op.i4 = k, stride, pad, side, side
             op.src0, op.w, op.bias, op.dst = src.data_ptr(), w.data_ptr(), b.data_ptr(), dst.data_ptr()

@@ -7,12 +7,15 @@ Three evaluation batches shaped like the outputs of the benchmark workloads, wit
   * cfg2: 64 clips x 20 frames, 64x64, 1 channel;
   * cfg4: 64 clips x 28 frames, 64x64, 3 channels;
   * cfg5: 32 clips x 28 frames, 128x128, 3 channels (the resize is an identity).
-``native`` is the whole ``LPIPS`` call (quantise, resize, AlexNet, heads) with the default chunk of 256 pairs.
+``native`` is the whole ``LPIPS`` call (quantise, resize, AlexNet, heads) with the default chunk of 256 pairs;
+``native_tf32`` is the same call with ``LPIPS(..., tf32=True)`` (the convolutions on the TF32 tensor cores).
 ``torchvision`` is ``alexnet().features[0:12]`` with the same weights plus the LPIPS head in torch, batched over all
 pairs of the batch (chunks of 256, like the native path), on the network input the native prep computed; its own
 input preparation is not timed, so it is a lower bound on that path.  It runs with TF32 off and on.
-Both are timed with CUDA events after a warm-up, alternated ``--reps`` times; the median is reported.
-Prints the GPU's name and power limit, then one JSON line per case.
+All are timed with CUDA events after a warm-up, alternated ``--reps`` times; the median is reported.  Each case
+also reports the largest relative difference of the native fp32 and TF32 distances from torchvision's fp32 ones, of
+the TF32 distances from the native fp32 ones, and of torchvision's TF32 distances from its fp32 ones.  Prints the
+GPU's name and power limit, then one JSON line per case.
 """
 import argparse
 import json
@@ -74,6 +77,7 @@ def main():
     print(f"# {torch.cuda.get_device_name(dev)}, power limit {power_limit_w()} W")
     sd = LO.synthetic_weights()
     net = LP.LPIPS(sd, device=dev)
+    net_tf32 = LP.LPIPS(sd, device=dev, tf32=True)
     tv, lin = LO.torchvision_format(sd)
     alex = torchvision.models.alexnet(weights=None)
     alex.features.load_state_dict({k[len("features."):]: v for k, v in tv.items()})
@@ -101,7 +105,7 @@ def main():
                 return torch.cat([torchvision_lpips(features, lins, a, b) for a, b in inputs])
 
         res = {"case": name, "clips": B, "frames": F, "side": S, "channels": C, "pairs": N}
-        runs = {"native": lambda: net(pred, real, C)}
+        runs = {"native": lambda: net(pred, real, C), "native_tf32": lambda: net_tf32(pred, real, C)}
         for tf32 in (False, True):
             runs[f"torchvision_tf32_{'on' if tf32 else 'off'}"] = (lambda t=tf32: (
                 setattr(torch.backends.cudnn, "allow_tf32", t), setattr(torch.backends.cuda.matmul, "allow_tf32", t),
@@ -117,9 +121,18 @@ def main():
             res[f"{k}_ms"] = round(ms, 3)
             res[f"{k}_pairs_per_s"] = round(N / ms * 1e3, 1)
         d_native = net(pred, real, C).reshape(-1).double()
+        d_tf32 = net_tf32(pred, real, C).reshape(-1).double()
+        torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = True
+        d_tv_tf32 = tv_run().reshape(-1).double()
         torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
         d_tv = tv_run().reshape(-1).double()
-        res["max_rel_diff_vs_torchvision_fp32"] = float(((d_native - d_tv).abs() / d_tv.abs()).max())
+
+        def max_rel(a, b):
+            return float(((a - b).abs() / b.abs()).max())
+        res["max_rel_diff_vs_torchvision_fp32"] = max_rel(d_native, d_tv)
+        res["tf32_max_rel_diff_vs_torchvision_fp32"] = max_rel(d_tf32, d_tv)
+        res["tf32_max_rel_diff_vs_native_fp32"] = max_rel(d_tf32, d_native)
+        res["torchvision_tf32_max_rel_diff_vs_torchvision_fp32"] = max_rel(d_tv_tf32, d_tv)
         print(json.dumps(res), flush=True)
 
 
