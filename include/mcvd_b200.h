@@ -128,8 +128,8 @@ enum {
    * S and O in registers); same fields plus dst2 = device scratch of at least
    * mcvd_attention_scratch_bytes(B, H*W, C0) bytes (16-byte aligned): a first kernel splits q, k, v into
    * fp16 hi/lo operand images there, the attention kernel streams them in with cp.async.bulk (2 launches).
-   * Head dim in {32,48,64,96,128,192}, H*W a multiple of the key tile (128; 64 for head dim 128; 32 for head
-   * dim 192; H*W itself when smaller).  See mcvd_b200/csrc/attention_umma.cu. */
+   * Head dim in {32,48,64,96,128,192,256,288}, H*W a multiple of the key tile (128; 64 for head dim 128; 32 for
+   * head dims 192..288; H*W itself when smaller): mcvd_attention_key_tile.  See mcvd_b200/csrc/attention_umma.cu. */
   MCVD_OP_ATTENTION_UMMA = 15,
   /* MCVD_OP_CONV_UMMA with the norm table in planar form (same wgmma kernel, mcvd_b200/csrc/conv_umma.cu).  Same
    * semantics and fields, except:
@@ -390,6 +390,10 @@ long long mcvd_tf32_packed_bytes(int K, int Cout);
 int mcvd_tf32_pack_weights(const float* w_kmajor, int K, int Cout, void* out, void* stream);
 /* Bytes of dst2 scratch one MCVD_OP_ATTENTION_UMMA op with batch B, T = H*W tokens and C channels needs. */
 long long mcvd_attention_scratch_bytes(int B, int T, int C);
+/* Key tile the kernel of `kind` (MCVD_OP_ATTENTION or MCVD_OP_ATTENTION_UMMA) runs T = H*W tokens at head dim d
+ * (i1) with; 0 when it is not built for that head dim, or (tensor cores) T is not a whole number of its key tiles.
+ * An op of that kind and shape is launchable exactly when this is > 0. */
+int mcvd_attention_key_tile(int kind, int T, int d);
 
 #ifdef __cplusplus
 }

@@ -82,6 +82,15 @@ def check_supported(config) -> Optional[str]:
         return "ngf must be a multiple of 16"
     if d.image_size % (2 ** (len(m.ch_mult) - 1)) != 0:
         return "image_size not divisible by the down-sampling factor"
+    try:
+        spec = build_spec(config)
+    except AssertionError as e:
+        return str(e)
+    from . import lib                            # the attention kernels say which head dims they are built for
+    for ms in spec.mods:
+        if ms.kind == "attn" and lib.attention_kind(ms.res * ms.res, ms.in_ch // ms.heads) is None:
+            return (f"attention head dim {ms.in_ch // ms.heads} ({ms.heads} heads x {ms.in_ch // ms.heads} at "
+                    f"{ms.res}x{ms.res}) has no native kernel")
     return None
 
 

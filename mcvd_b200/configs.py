@@ -65,13 +65,19 @@ def _mk(name, batch, data=None, model=None, sampling=None):
 
 
 def workload(name: str) -> argparse.Namespace:
-    """Return one of the benchmark workloads (``cfg1`` .. ``cfg5``) or a small test config.
+    """Return one of the benchmark workloads (``cfg1`` .. ``cfg7``) or a small test config.
 
     cfg1  smmnist_DDPM_small5.yml + model.arch=unetmore, subsample=10, B=2
     cfg2  smmnist_DDPM_big5.yml   + ngf=96 n_head_channels=96, subsample=100, B=64   (the headline)
     cfg3  kth64_big_spade.yml     + ngf=128 n_head_channels=128 spade_dim=128, B=32
     cfg4  bair_big.yml            + ngf=192 n_head_channels=192, B=64, num_frames_pred=28
     cfg5  cityscapes_big.yml      + ch_mult=[1,2,3,4,4], subsample=1000, B=32, num_frames_pred=28
+    cfg6  ucf101.yml              + ngf=288 n_head_channels=288, subsample=100, B=60, num_frames_pred=16
+                                    (ucf10132_big288_4c4_unetm: head dim 288)
+    cfg7  cityscapes_big.yml      + spade=True spade_dim=128 ngf=256 n_head_channels=256, subsample=100, B=32,
+                                    num_frames_pred=28 (city16_big128_256_5c2_unetm_long_spade: head dim 256; the
+                                    recipe samples 45 clips, but the lowered program keeps ~1.7 GiB of activation
+                                    buffers per clip, so 45 do not fit in 80 GB)
     """
     if name == "cfg1":
         return _mk(name, 2, data=dict(num_frames=2),
@@ -91,6 +97,15 @@ def workload(name: str) -> argparse.Namespace:
                    model=dict(depth="deeper", dropout=0.0, ngf=128, n_head_channels=128,
                               ch_mult=[1, 2, 3, 4, 4]),
                    sampling=dict(num_frames_pred=28, subsample=1000))
+    if name == "cfg6":
+        return _mk(name, 60, data=dict(channels=3, num_frames=4, num_frames_cond=4),
+                   model=dict(depth="deeper", ngf=288, n_head_channels=288),
+                   sampling=dict(num_frames_pred=16))
+    if name == "cfg7":
+        return _mk(name, 32, data=dict(image_size=128, channels=3, num_frames=5, num_frames_cond=2),
+                   model=dict(depth="deeper", dropout=0.0, ngf=256, n_head_channels=256, ch_mult=[1, 1, 2, 3, 4],
+                              spade=True, spade_dim=128),
+                   sampling=dict(num_frames_pred=28))
     # --- small configurations used by the parity tests (oracle finishes in seconds) ---
     if name == "tiny":      # concat conditioning, every block type, 32x32
         return _mk(name, 2, data=dict(image_size=32, num_frames=2, num_frames_cond=3),
@@ -127,5 +142,5 @@ def workload(name: str) -> argparse.Namespace:
     raise KeyError(f"unknown workload {name!r}")
 
 
-ALL_WORKLOADS = ("cfg1", "cfg2", "cfg3", "cfg4", "cfg5")
+ALL_WORKLOADS = ("cfg1", "cfg2", "cfg3", "cfg4", "cfg5", "cfg6", "cfg7")
 TEST_WORKLOADS = ("tiny", "tiny_spade", "tiny_rgb", "tiny128", "tiny_general", "tiny_spade_general", "tiny_gamma")

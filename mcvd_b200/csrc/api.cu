@@ -264,6 +264,12 @@ int mcvd_count_launches(const McvdOp* ops, int n) {
   return total;
 }
 
+int mcvd_attention_key_tile(int kind, int T, int d) {
+  if (kind == MCVD_OP_ATTENTION) return mcvd::attention_simt_key_tile(T, d);
+  if (kind == MCVD_OP_ATTENTION_UMMA) return mcvd::attention_umma_key_tile(T, d);
+  return 0;
+}
+
 int mcvd_run_program(const McvdOp* ops, int n, void* stream) {
   if (!ops || n < 0) {
     mcvd::set_error("null program");

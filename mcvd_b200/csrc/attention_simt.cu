@@ -175,6 +175,14 @@ int launch_one(const McvdOp& op, cudaStream_t s) {
 
 }  // namespace
 
+// the head dims launch_attention runs; any T (the last key tile is partial)
+int attention_simt_key_tile(int T, int d) {
+  switch (d) {
+    case 16: case 32: case 48: case 64: case 96: case 128: case 192: case 256: return T > 0 ? TK : 0;
+    default: return 0;
+  }
+}
+
 int launch_attention(const McvdOp& op, cudaStream_t s) {
   MCVD_CHECK(op.src0 && op.dst, "ATTENTION: null pointer");
   int d = op.i1, heads = op.i0;

@@ -9,7 +9,8 @@
 //                 S = Q K^T   (wgmma m64nKTk16, both operands from shared memory)   -> registers
 //                 P = exp(S*scale - m), online max / sum in registers (a row lives in the 4 lanes of a quad)
 //                 O = O * exp(m_old - m_new) + P V   (wgmma m64nDk16, P from registers: the fp32 accumulator
-//                     layout of S is the register A-operand layout, so P never touches shared memory)
+//                     layout of S is the register A-operand layout, so P never touches shared memory; wgmma's
+//                     N stops at 256, so head dim 288 issues it as two N = 144 halves of the channels)
 // fp32 parity: q, k, v and p are split into fp16 hi + lo and every product is 3 MMAs
 // (hi*hi + lo*hi + hi*lo), fp32 accumulation -- same scheme as conv_umma.cu.
 //
@@ -32,6 +33,12 @@ using namespace ptx;
 
 constexpr int QT = 128;
 constexpr int ATT_THREADS = 288;       // 2 consumer warpgroups + image loader
+// Head dims 256 / 288 hold 128 / 144 O accumulators per consumer thread, more than the 168 registers a 288- or
+// 384-thread CTA gets.  There the loader is a whole warpgroup that hands registers to the consumers (setmaxnreg):
+// 2 x 128 x 232 + 128 x 40 <= 64 K.
+template <int D> __host__ __device__ constexpr bool wide_head() { return D > 192; }
+template <int D> __host__ __device__ constexpr int att_threads() { return wide_head<D>() ? 384 : ATT_THREADS; }
+constexpr int REG_LOAD_WIDE = 40, REG_CONS_WIDE = 232;
 constexpr int SPLIT_THREADS = 256;
 
 struct AttnArgs {
@@ -126,8 +133,16 @@ __device__ __forceinline__ void stage_v(uint8_t* vh, uint8_t* vl, const float* v
   }
 }
 
-// key tile: as large as the operand images allow in shared memory (Q is resident: 4*D*128 bytes)
+// key tile: as large as the operand images allow in shared memory (Q is resident: 4*D*128 bytes).  Head dims 256
+// and 288 (128 / 144 KiB of Q) fit one K + V^T stage of 32 keys (64 / 72 KiB), not two: see launch_d.
 template <int D> __host__ __device__ constexpr int kt_max() { return D <= 96 ? 128 : (D <= 128 ? 64 : 32); }
+
+// the key tile a T-token attention runs with (T itself when smaller than kt_max), 0 when T is not a whole number
+// of key tiles the kernel is built for.  The lowering asks for it through mcvd_attention_key_tile.
+template <int D> int key_tile(int T) {
+  const int kt = T < kt_max<D>() ? T : kt_max<D>();
+  return ((kt == 32 || kt == 64 || kt == 128) && T % kt == 0) ? kt : 0;
+}
 
 // image sizes in bytes (hi plane + lo plane)
 template <int D> __host__ __device__ constexpr long long q_image_bytes() { return 2LL * (D / 8) * QT * 16; }
@@ -158,10 +173,25 @@ __global__ void __launch_bounds__(SPLIT_THREADS) k_attn_presplit(const AttnArgs 
   }
 }
 
-// Attention kernel: grid (nqt, heads, B), 288 threads.  Warps 0-7 = two consumer warpgroups (query rows
-// [64 wg, 64 wg + 64) of the tile), warp 8 = image loader (Q once, then K / V^T tiles through NST stages).
+// O += P V over one 16-key step: head dims up to 256 in one wgmma, 288 as two N = 144 halves (V^T rows =
+// channels at 16 B, so the second half starts D/2 rows in; its accumulators are o[D/4 ..)).  Every output
+// element still sums the same products in the same order.
+template <int D>
+__device__ __forceinline__ void wgmma_pv(float* o, const uint32_t* p, uint64_t v) {
+  if constexpr (D <= 256) {
+    wgmma_rs<D>(o, p, v);
+  } else {
+    wgmma_rs<D / 2>(o, p, v);
+    wgmma_rs<D / 2>(o + D / 4, p, desc_add(v, D / 2));
+  }
+}
+
+// Attention kernel: grid (nqt, heads, B), att_threads<D>() threads.  Warps 0-7 = two consumer warpgroups (query
+// rows [64 wg, 64 wg + 64) of the tile), warp 8 = image loader (Q once, then K / V^T tiles through NST stages);
+// warps 9-11 (wide heads only) just give their registers away.
 template <int D, int KT>
-__global__ void __launch_bounds__(ATT_THREADS, 1) k_attention_umma(const AttnArgs a) {
+__global__ void __launch_bounds__(att_threads<D>(), 1) k_attention_umma(const AttnArgs a) {
+  constexpr bool WIDE = wide_head<D>();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int NQ = QT / 64;                 // consumer warpgroups
   const int NST = a.nst;
@@ -191,9 +221,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) k_attention_umma(const AttnArg
   }
   __syncthreads();
 
-  if (warp == 4 * NQ) {
+  if (WIDE ? warp >= 4 * NQ : warp == 4 * NQ) {
     // ================= image loader =================
-    if (elect_one()) {
+    if constexpr (WIDE) setmaxnreg_dec<REG_LOAD_WIDE>();
+    if ((!WIDE || warp == 4 * NQ) && elect_one()) {
       mbar_arrive_expect_tx(Q_FULL, q_bytes);
       bulk_g2s(smem_u32(qimg), a.img + (bh * a.nqt + blockIdx.x) * q_image_bytes<D>(), q_bytes, Q_FULL);
       for (int kt = 0; kt < a.nkt; ++kt) {
@@ -213,6 +244,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) k_attention_umma(const AttnArg
   }
 
   // ================= consumers: S = Q K^T, online softmax, O += P V =================
+  if constexpr (WIDE) setmaxnreg_inc<REG_CONS_WIDE>();
   const int wg = warp >> 2, wq = warp & 3;
   const int r0 = 64 * wg + 16 * wq + (lane >> 2);          // query rows r0 and r0 + 8 of the tile
   const int cq = 2 * (lane & 3);
@@ -288,9 +320,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) k_attention_umma(const AttnArg
 #pragma unroll
     for (int kk = 0; kk < KT / 16; ++kk) {
       const uint64_t vh = desc_add(v_desc, 2u * kk * D), vl = desc_add(vh, kv_lo16);
-      wgmma_rs<D>(o, ph4[kk], vh);
-      wgmma_rs<D>(o, pl4[kk], vh);
-      wgmma_rs<D>(o, ph4[kk], vl);
+      wgmma_pv<D>(o, ph4[kk], vh);
+      wgmma_pv<D>(o, pl4[kk], vh);
+      wgmma_pv<D>(o, ph4[kk], vl);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -323,7 +355,7 @@ int launch_dk(const AttnArgs& a, size_t smem, const McvdOp& op, cudaStream_t s) 
   k_attn_presplit<D><<<sgrid, SPLIT_THREADS, 0, s>>>(a);
   MCVD_CUDA_LAUNCH_CHECK("attention presplit");
   dim3 grid(a.nqt, op.i0, op.B);
-  k_attention_umma<D, KT><<<grid, ATT_THREADS, smem, s>>>(a);
+  k_attention_umma<D, KT><<<grid, att_threads<D>(), smem, s>>>(a);
   MCVD_CUDA_LAUNCH_CHECK("attention_umma");
   return 0;
 }
@@ -333,10 +365,8 @@ int launch_d(const McvdOp& op, cudaStream_t s) {
   AttnArgs a;
   a.qkv = (const float*)op.src0; a.out = (float*)op.dst;
   a.T = op.H * op.W; a.C = op.C0; a.scale = op.f0;
-  a.KT = kt_max<D>();
-  if (a.T < a.KT) a.KT = a.T;
-  MCVD_CHECK((a.KT == 32 || a.KT == 64 || a.KT == 128) && a.T % a.KT == 0,
-             "ATTENTION_UMMA: %d tokens not tileable by the key tile %d", a.T, a.KT);
+  a.KT = key_tile<D>(a.T);
+  MCVD_CHECK(a.KT > 0, "ATTENTION_UMMA: %d tokens not tileable by the key tile %d", a.T, min(a.T, kt_max<D>()));
   a.nkt = a.T / a.KT;
   a.nqt = cdiv(a.T, QT);
   a.img = (uint8_t*)op.dst2;
@@ -345,7 +375,8 @@ int launch_d(const McvdOp& op, cudaStream_t s) {
   a.v_off = a.k_off + bh * a.nkt * kv_image_bytes<D>(a.KT);
   MCVD_CHECK(op.dst2, "ATTENTION_UMMA: dst2 (operand-image scratch, mcvd_attention_scratch_bytes) is NULL");
   MCVD_CHECK((reinterpret_cast<uintptr_t>(op.dst2) & 15) == 0, "ATTENTION_UMMA: scratch must be 16-byte aligned");
-  // Q stays resident; K and V^T tiles are double-buffered when two stages fit
+  // Q stays resident; K and V^T tiles are double-buffered when two stages fit (head dims up to 192).  At 256 / 288
+  // one stage: the loader refills K while the consumers run the softmax and P V, and V^T while they run the next S.
   const size_t q_bytes = (size_t)q_image_bytes<D>(), kv_bytes = (size_t)kv_image_bytes<D>(a.KT);
   a.nst = (q_bytes + 4 * kv_bytes + 128 <= 227 * 1024) ? 2 : 1;
   const size_t smem = q_bytes + 2 * a.nst * kv_bytes + 128;
@@ -365,6 +396,22 @@ long long attention_umma_scratch_bytes(int B, int T, int C) {
   return 4LL * B * C * ((long long)cdiv(T, QT) * QT + 2LL * T);
 }
 
+// the head dims the kernel is built for, with the key tile of T tokens (0: not built for d, or T not tileable)
+int attention_umma_key_tile(int T, int d) {
+  if (T <= 0) return 0;
+  switch (d) {
+    case 32: return key_tile<32>(T);
+    case 48: return key_tile<48>(T);
+    case 64: return key_tile<64>(T);
+    case 96: return key_tile<96>(T);
+    case 128: return key_tile<128>(T);
+    case 192: return key_tile<192>(T);
+    case 256: return key_tile<256>(T);
+    case 288: return key_tile<288>(T);
+    default: return 0;
+  }
+}
+
 int launch_attention_umma(const McvdOp& op, cudaStream_t s) {
   MCVD_CHECK(op.src0 && op.dst, "ATTENTION_UMMA: null pointer");
   MCVD_CHECK(op.i0 * op.i1 == op.C0, "ATTENTION_UMMA: heads %d x dim %d != channels %d", op.i0, op.i1, op.C0);
@@ -375,9 +422,11 @@ int launch_attention_umma(const McvdOp& op, cudaStream_t s) {
     case 96: return launch_d<96>(op, s);
     case 128: return launch_d<128>(op, s);
     case 192: return launch_d<192>(op, s);          // cfg4 (bair_big, n_head_channels = 192): key tile 32
+    case 256: return launch_d<256>(op, s);          // cfg7 (Cityscapes SPADE, n_head_channels = 256): one stage
+    case 288: return launch_d<288>(op, s);          // cfg6 (UCF-101, n_head_channels = 288): one stage, split P V
     default: break;
   }
-  set_error("ATTENTION_UMMA: head dim %d unsupported (32/48/64/96/128/192)", op.i1);
+  set_error("ATTENTION_UMMA: head dim %d unsupported (32/48/64/96/128/192/256/288)", op.i1);
   return -1;
 }
 

@@ -59,6 +59,9 @@ int launch_conv_umma2(const McvdOp& op, cudaStream_t s);
 int launch_conv_smalln(const McvdOp& op, cudaStream_t s);
 int launch_copy(const McvdOp& op, cudaStream_t s);
 int launch_attention_umma(const McvdOp& op, cudaStream_t s);
+// key tile the attention kernels run T tokens at head dim d with; 0 where they are not built for the shape
+int attention_simt_key_tile(int T, int d);
+int attention_umma_key_tile(int T, int d);
 int launch_frame_metrics(const McvdOp& op, cudaStream_t s);
 int launch_noise(const McvdOp& op, cudaStream_t s);
 int launch_lpips_prep(const McvdOp& op, cudaStream_t s);

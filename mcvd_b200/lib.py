@@ -69,7 +69,7 @@ ABI_VERSION = 5
 EXPORTS = ["mcvd_abi_version", "mcvd_sizeof_op", "mcvd_last_error", "mcvd_device_arch", "mcvd_run_program",
            "mcvd_validate_program", "mcvd_count_launches", "mcvd_umma_pack_weights", "mcvd_umma_pack_weights_ex", "mcvd_umma_kblock",
            "mcvd_attention_scratch_bytes", "mcvd_umma2_plan", "mcvd_umma2_plan_info", "mcvd_conv_umma_launch_info", "mcvd_umma2_stats_bytes", "mcvd_umma2_pack_weights",
-           "mcvd_tf32_packed_bytes", "mcvd_tf32_pack_weights"]
+           "mcvd_tf32_packed_bytes", "mcvd_tf32_pack_weights", "mcvd_attention_key_tile"]
 
 
 class McvdOp(C.Structure):
@@ -141,6 +141,8 @@ def load():
         lib.mcvd_umma_kblock.argtypes = [C.c_int, C.c_int]
         lib.mcvd_attention_scratch_bytes.restype = C.c_longlong
         lib.mcvd_attention_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        lib.mcvd_attention_key_tile.restype = C.c_int
+        lib.mcvd_attention_key_tile.argtypes = [C.c_int, C.c_int, C.c_int]
         lib.mcvd_umma2_plan.restype = C.c_int
         lib.mcvd_umma2_plan.argtypes = [C.c_int] * 9
         lib.mcvd_umma2_plan_info.restype = C.c_int
@@ -193,6 +195,19 @@ def umma_kblock(c0: int, c1: int) -> int:
 def attention_scratch_bytes(B: int, T: int, C: int) -> int:
     """bytes of ``dst2`` scratch an OP_ATTENTION_UMMA op needs (fp16 hi/lo operand images of q, k, v)"""
     return int(load().mcvd_attention_scratch_bytes(B, T, C))
+
+
+def attention_kind(T: int, d: int, mode: str = "umma"):
+    """the op kind that runs an attention over T tokens at head dim d: OP_ATTENTION_UMMA in mode 'umma' where the
+    tensor-core kernel is built for the head dim and T is a whole number of its key tiles, else OP_ATTENTION where
+    the CUDA-core kernel is built for the head dim; None when no kernel runs it.  The library answers
+    (mcvd_attention_key_tile), so the lowering and the support check cannot drift from the kernels' own rules."""
+    L = load()
+    if mode == "umma" and L.mcvd_attention_key_tile(OP_ATTENTION_UMMA, T, d) > 0:
+        return OP_ATTENTION_UMMA
+    if L.mcvd_attention_key_tile(OP_ATTENTION, T, d) > 0:
+        return OP_ATTENTION
+    return None
 
 
 def umma2_plan(H: int, W: int, ks: int, c0: int, c1: int, c2: int, c3: int, n_tile: int, stats: bool) -> int:

@@ -648,9 +648,11 @@ class Engine:
             att = f32(B, H, H, C)
             d = C // ms.heads
             T = H * H
-            kt = min(T, 128 if d <= 96 else (64 if d <= 128 else 32))
-            use_tc = self.attn_mode == "umma" and d in (32, 48, 64, 96, 128, 192) and T % kt == 0 and kt in (32, 64, 128)
-            if use_tc:
+            kind = lib.attention_kind(T, d, self.attn_mode)
+            if kind is None:
+                raise ValueError(f"mcvd_b200: no {self.attn_mode} attention kernel for head dim {d} "
+                                 f"({ms.heads} heads x {d} = {C} channels, {H}x{H} tokens, module {ms.idx})")
+            if kind == lib.OP_ATTENTION_UMMA:
                 # q/k/v operand images (fp16 hi/lo); one scratch serves every attention layer (stream order)
                 need = lib.attention_scratch_bytes(B, T, C)
                 if attn_scratch[0] is None or attn_scratch[0].numel() < need:
