@@ -76,8 +76,9 @@ def workload(name: str) -> argparse.Namespace:
                                     (ucf10132_big288_4c4_unetm: head dim 288)
     cfg7  cityscapes_big.yml      + spade=True spade_dim=128 ngf=256 n_head_channels=256, subsample=100, B=32,
                                     num_frames_pred=28 (city16_big128_256_5c2_unetm_long_spade: head dim 256; the
-                                    recipe samples 45 clips, but the lowered program keeps ~1.7 GiB of activation
-                                    buffers per clip, so 45 do not fit in 80 GB)
+                                    recipe samples 45 clips: with liveness-planned activations the program needs
+                                    ~0.9 GiB per clip, so 45 fit on an 80 GB card (``bench.py --batch 45``); the
+                                    bench batch stays 32 so earlier measurements remain comparable)
     """
     if name == "cfg1":
         return _mk(name, 2, data=dict(num_frames=2),

@@ -2,8 +2,8 @@
 
 ``Engine`` owns, per module instance: the packed weights (repacked lazily when a parameter's version
 counter changes -- ``load_state_dict`` / ``EMAHelper.ema`` modify parameters after construction), and
-one ``Program`` per batch size: statically allocated NHWC activation buffers plus three ctypes op
-arrays
+one ``Program`` per batch size: one activation arena, in which the NHWC buffers are placed by live interval
+(``plan_buffers``, mcvd_b200/memplan.py), plus three ctypes op arrays
 
   * ``cond_ops``  -- everything that depends on ``cond`` only (SPADE: the 3 conv3x3 per norm that
                      produce gamma/beta, reference layerspp.py:165-168; they are independent of t and
@@ -24,7 +24,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from . import arch, lib
+from . import arch, lib, memplan
 from .lib import McvdOp
 
 INV_SQRT2 = float(1.0 / math.sqrt(2.0))
@@ -54,6 +54,123 @@ def _ptr(t) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+class VBuf:
+    """An activation buffer during lowering: shape, element type and a unique placeholder address.  Its place in the
+    program's arena is known only after every op is emitted (mcvd_b200/memplan.py); ``_build`` then patches the op
+    pointers.  ``data_ptr()`` returns the placeholder, so buffers keep their identity in the lowering's dicts.
+    ``own``: the buffer is a ``Program`` attribute the host reads or writes; it gets its own allocation, so a tensor
+    handed to a caller never keeps the whole arena alive.  ``held``: a temporary that stays live to the end of the
+    step program."""
+    _next = 1 << 48                              # above every user-space address: never a real pointer
+
+    def __init__(self, shape, dtype, own=False):
+        self.shape = tuple(int(s) for s in shape)
+        self.dtype = dtype
+        self.nbytes = math.prod(self.shape) * torch.empty((), dtype=dtype).element_size()
+        self.own = self.persistent = own
+        self.held = False
+        self.placeholder = VBuf._next
+        VBuf._next += 1 << 12
+        self.offset = None
+
+    def data_ptr(self) -> int:
+        return self.placeholder
+
+
+def _stat_tiles(B: int, H: int, W: int, ks: int) -> int:
+    """(tiles x image slots) of the conv-epilogue statistics of a ks x ks conv (include/mcvd_b200.h)"""
+    pimg = (H + 1) * (W + 1) if ks == 3 else H * W
+    return 2 * ((B * pimg + 255) // 256) * (127 // pimg + 2)
+
+
+def op_extents(op) -> List[Tuple[str, int, torch.dtype, bool]]:
+    """(pointer field, elements, element type, written) of every activation buffer an op of the score-network
+    program reads or writes, as its kind implies (include/mcvd_b200.h).  Weights and biases are not listed."""
+    k, B, H, W = op.kind, op.B, op.H, op.W
+    f32, f64, i64 = torch.float32, torch.float64, torch.int64
+    out: List[Tuple[str, int, torch.dtype, bool]] = []
+
+    def r(f, n, dt=f32):
+        if getattr(op, f):
+            out.append((f, n, dt, False))
+
+    def w(f, n, dt=f32):
+        if getattr(op, f):
+            out.append((f, n, dt, True))
+
+    if k == lib.OP_NCHW_TO_NHWC:
+        r("src0", B * op.C0 * H * W)
+        r("src1", B * op.C1 * H * W)
+        w("dst", B * H * W * (op.Cout if op.Cout > 0 else op.C0 + op.C1))
+    elif k == lib.OP_NHWC_TO_NCHW:
+        r("src0", B * H * W * (op.C1 if op.C1 > 0 else op.C0))
+        w("dst", B * op.C0 * H * W)
+    elif k == lib.OP_TIMESTEP_EMBED:
+        r("src0", B)
+        w("dst", B * op.Cout)
+    elif k == lib.OP_LINEAR:
+        r("src0", B * op.C0)
+        w("dst", B * op.Cout)
+    elif k == lib.OP_GN_PARTIAL:
+        r("src0", B * H * W * op.C0)
+        r("src1", B * H * W * op.C1)
+        w("dst", B * op.i0 * (op.C0 + op.C1) * 2, f64)
+    elif k == lib.OP_GN_FINALIZE:
+        C = op.C0 + op.C1
+        for f, c, kind in (("src0", op.C0, op.i4), ("src1", op.C1, op.i5)):
+            if kind == 0:
+                r(f, B * op.i0 * c * 2, f64)
+            else:
+                r(f, _stat_tiles(B, H, W, kind) * 2 * c, i64)
+        if op.flags & lib.F_FILM:                # batch stride i2; 0: one row shared by every clip
+            r("aux0", B * op.i2 if op.i2 else op.i3 + 2 * C)
+        w("dst", B * C * 4)
+        w("dst2", B * 3 * C)
+    elif k == lib.OP_APPLY:
+        Hin, Win = (2 * H, 2 * W) if op.flags & lib.F_DOWN else ((H // 2, W // 2) if op.flags & lib.F_UP else (H, W))
+        C = op.C0 + op.C1
+        r("src0", B * Hin * Win * op.C0)
+        r("src1", B * Hin * Win * op.C1)
+        r("aux0", B * C * 4)
+        r("aux1", B * Hin * Win * C)
+        r("aux2", B * Hin * Win * C)
+        w("dst", B * H * W * C)
+        w("dst2", B * H * W * C)
+    elif k in (lib.OP_CONV_SIMT, lib.OP_CONV_UMMA, lib.OP_CONV_UMMA2, lib.OP_CONV_SMALLN):
+        C = op.C0 + op.C1
+        r("src0", B * H * W * op.C0)
+        r("src1", B * H * W * op.C1)
+        r("src2", B * H * W * op.C2)
+        r("src3", B * H * W * op.C3)
+        if k == lib.OP_CONV_SMALLN:
+            r("aux0", B * op.C0 * 4)
+        else:
+            r("aux0", B * H * W * op.Cout)
+            r("aux1", B * 3 * C if k == lib.OP_CONV_UMMA2 else B * C * 4)
+        w("dst", B * H * W * op.Cout)
+        if k in (lib.OP_CONV_UMMA, lib.OP_CONV_UMMA2):
+            w("dst2", _stat_tiles(B, H, W, op.i0) * 2 * op.Cout, i64)
+    elif k in (lib.OP_ATTENTION, lib.OP_ATTENTION_UMMA):
+        r("src0", B * H * W * 3 * op.C0)
+        if k == lib.OP_ATTENTION_UMMA:          # operand images: written by the pre-split, then read
+            w("dst2", lib.attention_scratch_bytes(B, H * W, op.C0), torch.uint8)
+        w("dst", B * H * W * op.C0)
+    elif k == lib.OP_RESIZE_NEAREST:
+        r("src0", B * op.i0 * op.i1 * op.C0)
+        w("dst", B * H * W * op.C0)
+    elif k == lib.OP_DIFFUSION_UPDATE:
+        r("src0", B * H * W * (op.Cout if op.Cout > 0 else op.C0))
+        r("src1", B * op.C0 * H * W)
+        r("dst", B * op.C0 * H * W)
+        w("dst", B * op.C0 * H * W)
+    elif k == lib.OP_COPY:
+        r("src0", op.i0)
+        w("dst", op.i0)
+    else:
+        raise NotImplementedError(f"op kind {k} is not part of the score-network program")
+    return out
+
+
 def umma_scale_log2(amax: float) -> int:
     """Power-of-two pre-scale k of a tensor-core conv's weights (the kernel multiplies by f1 = 2^-k afterwards):
     max|w| * 2^k lies in [256, 512), so the fp16 hi parts keep 11 bits and the lo parts stay in the fp16 normal range
@@ -73,9 +190,62 @@ def _pick_nt(cout: int) -> int:
     return best
 
 
+def plan_buffers(P, bufs: List[VBuf], refs) -> None:
+    """Place a lowered program's buffers (``bufs``; ``refs`` = (op, pointer field, buffer)) by live interval on the
+    timeline cond ops, then step ops, and check the plan.  The tensors the host reads or writes (``own`` buffers)
+    stay out of the arena.  Persistent, at the arena's front: every cond output a step op reads, since the cond ops
+    run once per sampler call and the step ops many times.  Every other buffer is a temporary, live from its first to
+    its last use (a ``held`` one to the last step op), whose first use must be a write.  Every op's extent
+    (``op_extents``) must fit inside the buffers it names, and buffers that start at one offset share type and size.
+    Sets ``offset`` of every arena buffer and P.io_bytes (the host's tensors), P.persistent_bytes, P.arena_bytes
+    (the temporaries' region), P.lower_bound_bytes (no placement of the temporaries needs less) and P.unplanned_bytes
+    (one allocation per buffer)."""
+    by_ptr = {v.placeholder: v for v in bufs}
+    named = {(id(o), f) for o, f, _ in refs}
+    n_cond = len(P.cond_ops)
+    uses: Dict[int, List[Tuple[int, bool]]] = {id(v): [] for v in bufs}
+    for pos, o in enumerate(P.cond_ops + P.step_ops):
+        listed = set()
+        for f, n, dt, written in op_extents(o):
+            v = by_ptr.get(getattr(o, f))
+            assert v is not None, f"op {pos} (kind {o.kind}).{f} names no activation buffer"
+            need = n * torch.empty((), dtype=dt).element_size()
+            assert need <= v.nbytes, f"op {pos} (kind {o.kind}).{f} spans {need} bytes of a {v.nbytes}-byte buffer"
+            uses[id(v)].append((pos, written))
+            listed.add(f)
+        for f in ("src0", "src1", "src2", "src3", "aux0", "aux1", "aux2", "dst", "dst2"):
+            assert (id(o), f) not in named or f in listed, f"op {pos} (kind {o.kind}).{f}: extent unknown"
+    intervals = []
+    placed = [v for v in bufs if not v.own]
+    for v in placed:
+        u = uses[id(v)]
+        if not v.persistent and u and min(p for p, _ in u) < n_cond <= max(p for p, _ in u):
+            v.persistent = True                                    # a cond output the step ops read
+        if v.persistent:
+            intervals.append(None)
+            continue
+        assert u, "a temporary buffer no op uses"
+        first = min(p for p, _ in u)
+        assert all(w for p, w in u if p == first), f"temporary first used by op {first} without being written"
+        intervals.append((first, n_cond + len(P.step_ops) - 1 if v.held else max(p for p, _ in u)))
+    sizes = [v.nbytes for v in placed]
+    kinds = [(str(v.dtype), v.nbytes) for v in placed]
+    offs, P.persistent_bytes, P.arena_bytes = memplan.place(sizes, intervals, kinds)
+    memplan.check(sizes, intervals, offs, kinds)
+    for v, off in zip(placed, offs):
+        v.offset = off
+    P.lower_bound_bytes = memplan.lower_bound(sizes, intervals)
+    P.io_bytes = sum(v.nbytes for v in bufs if v.own)
+    P.unplanned_bytes = sum(v.nbytes for v in bufs)
+
+
 class Program:
     def __init__(self):
-        self.keep: List[torch.Tensor] = []
+        self.keep: List[torch.Tensor] = []           # weights, biases and the arena the activations live in
+        self.arena: Optional[torch.Tensor] = None    # uint8: persistent buffers, then the temporaries' region
+        self.io_bytes = 0                            # inputs and outputs, allocated on their own
+        self.persistent_bytes = 0
+        self.arena_bytes = 0                         # bytes of the temporaries' region (mcvd_b200/memplan.py)
         self.cond_ops: List[McvdOp] = []
         self.step_ops: List[McvdOp] = []
         self.cond_arr = None
@@ -315,8 +485,8 @@ class Engine:
 
     # ------------------------------------------------------------------------------ lowering
     def program(self, B: int, check_weights: bool = True) -> Program:
-        """The lowered program for batch size B.  Every program owns its activation buffers (a few GB at the
-        benchmark batch sizes, mcvd_b200/configs.py), so only MAX_PROGRAMS are kept: uneven shards / last batches evict the least
+        """The lowered program for batch size B.  Every program owns its activation arena (up to tens of GB at
+        the benchmark batch sizes, README "Activation memory"), so only MAX_PROGRAMS are kept: uneven shards / last batches evict the least
         recently used one instead of piling up."""
         if B <= 0:
             raise ValueError(f"mcvd_b200: batch size {B} (an empty shard?) cannot be lowered")
@@ -349,7 +519,17 @@ class Engine:
         for v in self.packed.values():
             reg(v)
 
-    def _build(self, B: int) -> Program:
+    def plan(self, B: int) -> Program:
+        """The batch-B program lowered and its buffers placed, but nothing allocated: its ``arena_bytes``,
+        ``persistent_bytes`` and the other byte counts of ``plan_buffers``, without the memory.  Its ops hold
+        placeholder pointers and cannot run."""
+        if B <= 0:
+            raise ValueError(f"mcvd_b200: batch size {B} cannot be lowered")
+        self.ensure_packed()
+        with self._devctx():
+            return self._build(B, materialize=False)
+
+    def _build(self, B: int, materialize: bool = True) -> Program:
         ns = self.spec
         dev = self.device
         P = Program()
@@ -357,10 +537,16 @@ class Engine:
         P.conv_precision = self.conv_precision
         S = ns.image_size
 
+        bufs: List[VBuf] = []                        # every activation buffer, placed in the arena at the end
+        refs: List[Tuple[McvdOp, str, VBuf]] = []    # (op, pointer field, buffer) to patch once the plan is known
+
+        def vbuf(shape, dtype=torch.float32, own=False):
+            v = VBuf(shape, dtype, own)
+            bufs.append(v)
+            return v
+
         def f32(*shape):
-            t = torch.empty(shape, device=dev, dtype=torch.float32)
-            P.keep.append(t)
-            return t
+            return vbuf(shape)
 
         def keep(t):
             P.keep.append(t)
@@ -372,7 +558,10 @@ class Engine:
             o.B = B
             for k, v in kw.items():
                 if k in ("src0", "src1", "w", "bias", "aux0", "aux1", "aux2", "dst", "dst2", "src2", "src3"):
-                    if isinstance(v, torch.Tensor):
+                    if isinstance(v, VBuf):
+                        refs.append((o, k, v))
+                        v = v.placeholder
+                    elif isinstance(v, torch.Tensor):
                         v = v.data_ptr()
                     setattr(o, k, v)
                 else:
@@ -428,8 +617,7 @@ class Engine:
                         kw2 = dict(src2=sc_src.t0, src3=sc_src.t1, C2=c2, C3=c3)
                     st = None
                     if want_stats:
-                        st = keep(torch.zeros(lib.umma2_stats_bytes(B, H, H, ks, cout) // 8, device=dev,
-                                              dtype=torch.int64))
+                        st = vbuf((lib.umma2_stats_bytes(B, H, H, ks, cout) // 8,), torch.int64)
                         stats_of[dst.data_ptr()] = (st, ks)
                     emit(ops, lib.OP_CONV_UMMA2, H=H, W=H, C0=src.c0, C1=src.c1, Cout=cout, i0=ks, i1=nt, i2=kb,
                          i3=3 if half else self.split_mode, f0=scale, f1=wscale, src0=src.t0, src1=src.t1, w=wp, bias=bias,
@@ -467,7 +655,7 @@ class Engine:
                 st = None
                 pimg = (H + 1) * (H + 1) if ks == 3 else H * H
                 if stats and pimg >= 64 and self.epilogue_stats:   # GroupNorm partial sums from the epilogue
-                    st = keep(torch.zeros(lib.umma2_stats_bytes(B, H, H, ks, cout) // 8, device=dev, dtype=torch.int64))
+                    st = vbuf((lib.umma2_stats_bytes(B, H, H, ks, cout) // 8,), torch.int64)
                     stats_of[dst.data_ptr()] = (st, ks)
                 emit(ops, lib.OP_CONV_UMMA, H=H, W=H, C0=src.c0, C1=src.c1, Cout=cout, i0=ks, i1=nt, i2=nacc,
                      i3=3 if half else self.split_mode, f0=scale, f1=wscale, src0=src.t0, src1=src.t1, w=wp, bias=bias,
@@ -491,22 +679,21 @@ class Engine:
             return dst
 
         # ---- GroupNorm statistics -> (mean, rstd, G, S) table -----------------------------------
-        part_cache: Dict[int, torch.Tensor] = {}
+        part_cache: Dict[int, VBuf] = {}
 
-        def partials_of(ops, t: torch.Tensor, C: int, H: int, nchunk: int):
+        def partials_of(ops, t: VBuf, C: int, H: int, nchunk: int):
             """per-channel (sum, sum of squares) of one tensor, computed ONCE however many norms read it"""
             key = t.data_ptr()
             if key not in part_cache:
-                part = torch.empty(B * nchunk * C * 2, device=dev, dtype=torch.float64)
-                keep(part)
+                part = vbuf((B * nchunk * C * 2,), torch.float64)
                 emit(ops, lib.OP_GN_PARTIAL, H=H, W=H, C0=C, i0=nchunk, src0=t, dst=part)
                 part_cache[key] = part
             return part_cache[key]
 
-        stats_of: Dict[int, Tuple[torch.Tensor, int]] = {}     # tensor -> (conv-epilogue tile statistics, conv ks)
-        tab3_of: Dict[int, torch.Tensor] = {}                   # float4 table -> planar table (CONV_UMMA2 reads it)
+        stats_of: Dict[int, Tuple[VBuf, int]] = {}     # tensor -> (conv-epilogue tile statistics, conv ks)
+        tab3_of: Dict[int, VBuf] = {}                   # float4 table -> planar table (CONV_UMMA2 reads it)
 
-        def stat_source(ops, t: torch.Tensor, C: int, H: int, nchunk: int):
+        def stat_source(ops, t: VBuf, C: int, H: int, nchunk: int):
             """(array, kind): the producing conv's epilogue statistics (kind = its kernel size) when it wrote
             them, else the chunk partials of a separate pass over the tensor (kind 0)"""
             if t.data_ptr() in stats_of:
@@ -526,7 +713,7 @@ class Engine:
                 tab3_of[tab.data_ptr()] = f32(B, 3, C)
                 kw["dst2"] = tab3_of[tab.data_ptr()]
             if film_off is not None:
-                kw.update(aux0=P.film, i2=ns.film_total, i3=film_off, flags=lib.F_FILM)
+                kw.update(aux0=film, i2=ns.film_total, i3=film_off, flags=lib.F_FILM)
                 if ops is step:
                     P.film_fin_idx.append(len(ops))
             elif affine is not None:
@@ -535,15 +722,15 @@ class Engine:
             return tab
 
         # ---- SPADE gamma / beta (cond-only; reference layerspp.py:165-168) -------------------------
-        cond_at: Dict[int, torch.Tensor] = {}
+        cond_at: Dict[int, VBuf] = {}
 
         def cond_resized(H):
             if H not in cond_at:
                 if H == S:
-                    cond_at[H] = P.cond_nhwc
+                    cond_at[H] = cond_nhwc
                 else:
                     t = f32(B, H, H, ns.cond_ch)
-                    emit(cnd, lib.OP_RESIZE_NEAREST, H=H, W=H, C0=ns.cond_ch, i0=S, i1=S, src0=P.cond_nhwc, dst=t)
+                    emit(cnd, lib.OP_RESIZE_NEAREST, H=H, W=H, C0=ns.cond_ch, i0=S, i1=S, src0=cond_nhwc, dst=t)
                     cond_at[H] = t
             return cond_at[H]
 
@@ -558,19 +745,19 @@ class Engine:
             return g, b
 
         # ---- inputs ---------------------------------------------------------------------------------
-        P.x_in = f32(B, ns.out_ch, S, S)
-        P.cond_in = f32(B, ns.cond_ch, S, S) if ns.cond_ch > 0 else None
-        P.t = f32(B)
-        P.out = f32(B, ns.out_ch, S, S)
+        P.x_in = vbuf((B, ns.out_ch, S, S), own=True)
+        P.cond_in = vbuf((B, ns.cond_ch, S, S), own=True) if ns.cond_ch > 0 else None
+        P.t = vbuf((B,), own=True)
+        P.out = vbuf((B, ns.out_ch, S, S), own=True)
         # skinny first / last convs: zero-pad K (input channels) / N (output channels) to 16 so they run on the
         # tensor-core kernel instead of the CUDA-core ones
         tc_edges = self.conv_mode in ("umma", "umma2")
         in_pad = (ns.in_ch + 15) // 16 * 16 if tc_edges else ns.in_ch
         out_pad = (ns.out_ch + 15) // 16 * 16 if tc_edges else ns.out_ch
-        P.noise = f32(B, ns.out_ch, S, S)
+        P.noise = vbuf((B, ns.out_ch, S, S), own=True)
         if ns.spade:
-            P.cond_nhwc = f32(B, S, S, ns.cond_ch)
-            emit(cnd, lib.OP_NCHW_TO_NHWC, H=S, W=S, C0=ns.cond_ch, src0=P.cond_in, dst=P.cond_nhwc)
+            cond_nhwc = P.cond_nhwc = vbuf((B, S, S, ns.cond_ch), own=True)
+            emit(cnd, lib.OP_NCHW_TO_NHWC, H=S, W=S, C0=ns.cond_ch, src0=P.cond_in, dst=cond_nhwc)
             xin = f32(B, S, S, in_pad)
             emit(step, lib.OP_NCHW_TO_NHWC, H=S, W=S, C0=ns.out_ch, Cout=in_pad, src0=P.x_in, dst=xin)
         else:
@@ -581,7 +768,7 @@ class Engine:
         # ---- time embedding + all FiLM projections (ncsnpp_more.py:273-280; layerspp.py:521) --------
         mods = ns.mods
         emb, h0, temb = f32(B, ns.nf), f32(B, ns.temb_dim), f32(B, ns.temb_dim)
-        P.film = f32(B, ns.film_total)
+        film = P.film = vbuf((B, ns.film_total), own=True)
         P.temb_idx = list(range(len(step), len(step) + 4))
         emit(step, lib.OP_TIMESTEP_EMBED, Cout=ns.nf, src0=P.t, w=self.packed["freqs"], dst=emb)
         emit(step, lib.OP_LINEAR, C0=ns.nf, Cout=ns.temb_dim, src0=emb, w=keep(sd("unet.all_modules.0.weight").float().contiguous()),
@@ -590,10 +777,10 @@ class Engine:
              w=keep(sd("unet.all_modules.1.weight").float().contiguous()),
              bias=keep(sd("unet.all_modules.1.bias").float().contiguous()), dst=temb, flags=lib.F_ACT_OUT)
         emit(step, lib.OP_LINEAR, C0=ns.temb_dim, Cout=ns.film_total, src0=temb, w=self.packed["film_w"],
-             bias=self.packed["film_b"], dst=P.film)
+             bias=self.packed["film_b"], dst=film)
 
         # ---- blocks ---------------------------------------------------------------------------------
-        def resblock(ms: arch.ModSpec, src: Src) -> torch.Tensor:
+        def resblock(ms: arch.ModSpec, src: Src) -> VBuf:
             pre = f"unet.all_modules.{ms.idx}."
             Hin = ms.res
             H = Hin * 2 if ms.up else (Hin // 2 if ms.down else Hin)
@@ -634,9 +821,7 @@ class Engine:
             return conv(step, pre + "Conv_1", Src(h, Cout), H, Cout, 3, pre + "Conv_1.weight", pre + "Conv_1.bias",
                         residual=res, scale=INV_SQRT2, tab=tab1, act_in=True, shortcut=shortcut, stats=True)
 
-        attn_scratch = [None]
-
-        def attnblock(ms: arch.ModSpec, x: torch.Tensor) -> torch.Tensor:
+        def attnblock(ms: arch.ModSpec, x: VBuf) -> VBuf:
             pre = f"unet.all_modules.{ms.idx}."
             H, C = ms.res, ms.in_ch
             tab = norm_table(step, Src(x, C), H, 1e-6,
@@ -645,6 +830,9 @@ class Engine:
             bq = torch.cat([sd(pre + f"NIN_{i}.b").float() for i in range(3)], dim=0).contiguous()
             qkv = conv(step, pre + "qkv", Src(x, C), H, 3 * C, 1, None, None, tab=tab, act_in=False, nin=True, wcat=wq,
                        bcat=bq)
+            # q, k, v stay readable after a network evaluation, as they did with one allocation per buffer: the
+            # attention logits a run met can be inspected from P.keep (2-31 MiB per clip, README "Activation memory")
+            qkv.held = True
             att = f32(B, H, H, C)
             d = C // ms.heads
             T = H * H
@@ -653,12 +841,10 @@ class Engine:
                 raise ValueError(f"mcvd_b200: no {self.attn_mode} attention kernel for head dim {d} "
                                  f"({ms.heads} heads x {d} = {C} channels, {H}x{H} tokens, module {ms.idx})")
             if kind == lib.OP_ATTENTION_UMMA:
-                # q/k/v operand images (fp16 hi/lo); one scratch serves every attention layer (stream order)
-                need = lib.attention_scratch_bytes(B, T, C)
-                if attn_scratch[0] is None or attn_scratch[0].numel() < need:
-                    attn_scratch[0] = keep(torch.empty(need, device=dev, dtype=torch.uint8))
+                # q/k/v operand images (fp16 hi/lo): a temporary live within the op
+                scratch = vbuf((lib.attention_scratch_bytes(B, T, C),), torch.uint8)
                 emit(step, lib.OP_ATTENTION_UMMA, H=H, W=H, C0=C, i0=ms.heads, i1=d, f0=float(int(d) ** (-0.5)),
-                     src0=qkv, dst=att, dst2=attn_scratch[0])
+                     src0=qkv, dst=att, dst2=scratch)
             else:
                 emit(step, lib.OP_ATTENTION, H=H, W=H, C0=C, i0=ms.heads, i1=d, f0=float(int(d) ** (-0.5)),
                      src0=qkv, dst=att)
@@ -672,7 +858,7 @@ class Engine:
             w_first = wp_
         h = conv(step, "first", Src(xin, in_pad), S, ns.nf, 3, None, None, wcat=w_first,
                  bcat=sd("unet.all_modules.2.bias").float().contiguous(), stats=True)
-        hs: List[Tuple[torch.Tensor, int]] = [(h, ns.nf)]
+        hs: List[Tuple[VBuf, int]] = [(h, ns.nf)]
         cur, cur_c = h, ns.nf
         for ms in mods[3:-2]:
             if ms.kind == "res":
@@ -731,8 +917,31 @@ class Engine:
                 last_src = an
             emit(step, lib.OP_CONV_SIMT, H=S, W=S, C0=cur_c, Cout=ns.out_ch, i0=3, i1=coutp, f0=1.0, src0=last_src,
                  w=wlp, bias=bl, dst=P.eps_nhwc)
-        P.eps_nhwc.zero_()           # read (times 0) by the warm-start noising update before the first network call
+        P.eps_nhwc.own = P.eps_nhwc.persistent = True
         P.n_net_ops = len(step)
+        plan_buffers(P, bufs, refs)
+        if not materialize:
+            return P
+        raw = keep(torch.empty(P.persistent_bytes + P.arena_bytes + memplan.ALIGN, device=dev, dtype=torch.uint8))
+        skew = memplan.ALIGN - raw.data_ptr() % memplan.ALIGN     # >= 1: no buffer starts where the allocation does
+        P.arena = raw[skew:skew + P.persistent_bytes + P.arena_bytes]
+        own = {}
+        for name in ("x_in", "cond_in", "t", "out", "noise", "eps_nhwc", "film", "cond_nhwc"):
+            v = getattr(P, name, None)
+            if v is not None:
+                own[id(v)] = keep(torch.empty(v.shape, device=dev, dtype=v.dtype))
+                setattr(P, name, own[id(v)])
+        # one typed view per buffer start (memplan: buffers sharing a start share type and size), so P.keep resolves
+        # every op pointer to the buffer it names
+        starts = set()
+        for v in bufs:
+            if not v.own and v.offset not in starts:
+                starts.add(v.offset)
+                keep(P.arena[v.offset:v.offset + v.nbytes].view(v.dtype).view(v.shape))
+        base = P.arena.data_ptr()
+        for o, f, v in refs:
+            setattr(o, f, own[id(v)].data_ptr() if v.own else base + v.offset)
+        P.eps_nhwc.zero_()           # read (times 0) by the warm-start noising update before the first network call
 
         P.cond_arr = lib.make_ops(cnd) if cnd else None
         P.step_arr = lib.make_ops(step)
